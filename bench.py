@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native Bifrost hot path.
+"""bench.py -- headline benchmark of the H100-native (sm_90a) Bifrost hot path.
 
 Metric (BASELINE.json): Msamples/s through FDMT + FFT->detect->reduce on a
 4096-chan ci8/int8 stream, and % of the HBM roofline.
@@ -23,11 +23,14 @@ Metric (BASELINE.json): Msamples/s through FDMT + FFT->detect->reduce on a
          ranks including both collectives.  `replicas` keeps the weak-scaling
          figure (every rank its own full 4096-chan gulp, no collective).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 `--impl reference` times the CPU restatement of the reference algorithm
 (oracle/fdmt_c.c, all host threads) on a bounded sample of the same gulp.
 `--dry-run` exercises the multi-rank host logic on gloo with no GPU work.
+`--dump-outputs DIR` writes what the timed steps computed in their last step
+(a fixed sample of the dispersion bank and of the spectrometer output) as
+DIR/<name>.npy; the inputs are seeded, so two builds compare output for output.
 """
 import argparse
 import json
@@ -45,7 +48,7 @@ sys.path.insert(0, ROOT)
 NCHAN = 4096
 NTIME_OUT = 131072
 # bounded CPU sample, all 4096 channels: the whole gulp where the host has the cores to finish it
-# in well under a second (the B200 boxes: 128), else 1/4 of its time span (env override: tests only)
+# in well under a second (64 or more), else 1/4 of its time span (env override: tests only)
 def _mem_available_gb():
     try:
         for line in open('/proc/meminfo'):
@@ -102,7 +105,7 @@ def bench_config(world):
                              f'(max_delay={md}) on {NCHAN}-chan x {NTIME_OUT}(+{md})-sample '
                              'int8 filterbank; f0=1000 MHz, bw=400 MHz, dt=256 us',
                     sharding='single GPU',
-                    l2='input 540 MB + output 419 MB per step exceed the 126 MB L2')
+                    l2='input 540 MB + output 419 MB per step exceed the 50 MB L2')
     subs = [subband(g, world) for g in range(world)]
     nc = subs[0]['nchan']
     return dict(workload=f'BASELINE config 5: the one {NCHAN}-chan x {NTIME_OUT}(+{md})-sample int8 '
@@ -199,7 +202,8 @@ def measured_peaks():
             return json.load(open(path)), 'measured'
         except Exception:
             pass
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0), 'fallback'
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0), 'fallback (H100 SXM data sheet)'
 
 
 def bind_to_gpu_numa_node(index):
@@ -445,6 +449,8 @@ def main():
     ap.add_argument('--no-traffic', action='store_true')
     ap.add_argument('--no-gpu-reference', action='store_true')
     ap.add_argument('--dry-run', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write a fixed sample of what the last timed step computed as DIR/<name>.npy')
     ap.add_argument('--traffic-probe', action='store_true', help=argparse.SUPPRESS)
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'b200' else args.warmup
@@ -558,6 +564,8 @@ def main():
     ms_step = ms_total / args.steps
     launches_per_step = max(1, launches // args.steps)
     log('resident ms/step', ms_step)
+    if args.dump_outputs:
+        dump_bank(args.dump_outputs, np.asarray(d_out.copy('system')))
 
     # value check of exactly this gulp (untimed): five windows, both edges
     got_dev = d_out
@@ -567,7 +575,7 @@ def main():
     parity = oracle_window_check(x_host, got_fn, w, [(0, 4096), (40000, 4096), (65536 + 3, 4096), (100001, 4096),
                                                        (ntime - 4096 - md, 4096 + md)])
 
-    e2e_steps = max(4, min(args.steps, 10))
+    e2e_steps = args.steps
     ms_e2e_total, _, _ = timed(step_e2e, 2, e2e_steps)
     ms_e2e_serial = ms_e2e_total / e2e_steps
 
@@ -657,7 +665,7 @@ def main():
         traffic, traffic_how = measure_traffic(launches_per_step)
     roofline = dict(bound='hbm',
                     kernel=f'bfFdmtExecute = {launches_per_step} launch(es) per gulp (fdmt_packed*: packed-integer '
-                           'schedule, see DESIGN.md 4.1); bytes and time are those of the whole call',
+                           'schedule, see DESIGN.md §4); bytes and time are those of the whole call',
                     achieved=achieved, peak=peaks['hbm_gbs'], peak_source=peak_kind, unit='GB/s',
                     frac=achieved / peaks['hbm_gbs'], algorithmic_bytes=alg_bytes,
                     traffic=traffic, traffic_source=traffic_how,
@@ -672,7 +680,7 @@ def main():
     chain = None
     if not args.no_chain:
         del ws
-        chain = time_chain(bf, torch, timed, peaks)
+        chain = time_chain(bf, torch, timed, peaks, args)
 
     cpu = None
     if not args.no_cpu_baseline:
@@ -700,9 +708,22 @@ def main():
     print(json.dumps(line))
 
 
+def dump(dirname, name, arr):
+    os.makedirs(dirname, exist_ok=True)
+    arr = np.asarray(arr)
+    np.save(os.path.join(dirname, name + '.npy'), arr if arr.dtype == np.float64 else arr.astype(np.float32))
+
+
+def dump_bank(dirname, bank):
+    """All delay rows of a fixed sample of 4096 time columns of the dispersion
+    bank (13 MB of the 419 MB)."""
+    cols = np.sort(np.random.default_rng(1).choice(bank.shape[1], 4096, replace=False))
+    dump(dirname, 'fdmt_bank_sample', bank[:, cols])
+
+
 def time_gpu_reference(bf, torch, stream, d_in, d_out, w):
     """oracle/_ref/libbifrost_ref.so = the reference's own fdmt.cu compiled for
-    sm_100 (oracle/ref_build.sh): same device buffers, same stream."""
+    sm_90a (oracle/ref_build.sh): same device buffers, same stream."""
     import ctypes
     sys.path.insert(0, os.path.join(ROOT, 'tests'))
     try:
@@ -740,10 +761,11 @@ def time_gpu_reference(bf, torch, stream, d_in, d_out, w):
         return dict(available=False, note=f'reference library failed: {e}')
 
 
-def time_chain(bf, torch, timed, peaks):
+def time_chain(bf, torch, timed, peaks, args):
     nframe, cchan, nfft, f_avg = 32, 4096, 4096, 4
     nbyte = nframe * cchan * nfft * 4
-    raw = torch.randint(-127, 128, (nbyte,), dtype=torch.int8, device='cuda')
+    gen = torch.Generator(device='cuda').manual_seed(4321)
+    raw = torch.randint(-127, 128, (nbyte,), dtype=torch.int8, device='cuda', generator=gen)
     xg = bf.empty((nframe, cchan, nfft, 2), 'ci8', 'cuda')
     from bifrost_b200.libbifrost import _bf, _check
     _check(_bf.bfMemcpy(xg.ctypes.data, xg.as_BFarray().space, raw.data_ptr(),
@@ -751,13 +773,18 @@ def time_chain(bf, torch, timed, peaks):
     torch.cuda.synchronize()
     del raw
     og = bf.zeros((4, cchan * nfft // f_avg), 'f32', 'cuda')
-    ms_c, _, _ = timed(lambda: bf.spectrometer(xg, og, nfft, f_avg, 0.0), 3, 10)
-    ms_c /= 10
+    ms_c, _, _ = timed(lambda: bf.spectrometer(xg, og, nfft, f_avg, 0.0), args.warmup, args.steps)
+    ms_c /= args.steps
+    if args.dump_outputs:
+        out = np.asarray(og.copy('system'))
+        cols = np.sort(np.random.default_rng(2).choice(out.shape[1], 1 << 18, replace=False))
+        dump(args.dump_outputs, 'spectrometer_sample', out[:, cols])
     gbs = nbyte / (ms_c * 1e-3) / 1e9
     # useful fp32 work: 2 pols x 5 N log2 N per 4096-point FFT + detect/reduce (~16 flop/sample)
     flops = nframe * cchan * (2 * 5 * nfft * 12 + 16 * nfft)
     tflops = flops / (ms_c * 1e-3) / 1e12
-    fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12                 # SMs x lanes x FMA x GHz
+    # SMs x 128 FP32 lanes x 2 (FMA) x 1.98 GHz (H100 SXM boost clock)
+    fp32_peak = torch.cuda.get_device_properties(0).multi_processor_count * 128 * 2 * 1.98e9 / 1e12
     return dict(workload='BASELINE config 3: GUPPI ci8 [32 frames, 4096 chan, 4096 fine_time, 2 pol] -> '
                          'fft(fine_time, fftshift) -> stokes -> reduce(f_avg=4) -> accumulate(32 frames); '
                          'bfSpectrometerFused, one kernel per gulp',
@@ -818,6 +845,8 @@ def run_multi(args, rank, local_rank, world, bf, Fdmt, torch, dist, stream, time
 
     ms_total, launches, clocks = timed(step_strong, args.warmup, args.steps, sampler, post=compute)
     ms_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_bank(args.dump_outputs, t_bank.cpu().numpy())
     ms_scatter = timed(scatter, 2, 5)[0] / 5
     ms_compute = timed(compute, 2, 5)[0] / 5
     ms_gather = timed(gather, 2, 5)[0] / 5
@@ -900,7 +929,7 @@ def run_multi(args, rank, local_rank, world, bf, Fdmt, torch, dist, stream, time
             agree = torch.tensor([peer_ok], device='cuda')
             dist.all_reduce(agree, op=dist.ReduceOp.MIN)
             if int(agree.item()) == -1:
-                peer = dict(available=None, note='not requested (--fullband-peer); see profiles/r02_sharded_2gpu.txt')
+                peer = dict(available=None, note='not requested (--fullband-peer)')
             elif int(agree.item()) == 1:
                 peer_par = oracle_window_check(x_full, lambda a, n: t_fb[:, a:a + n].cpu().numpy(), full, wins) if rank == 0 else None
                 ms_peer = timed(lambda: sf.execute(x_loc, t_fb, peer=True), 2, 5)[0] / 5

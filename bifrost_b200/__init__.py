@@ -1,4 +1,4 @@
-"""bifrost_b200 -- B200-native (sm_100a) implementation of the Bifrost GPU DSP
+"""bifrost_b200 -- H100-native (sm_90a) implementation of the Bifrost GPU DSP
 hot path behind the reference's C ABI and ``bifrost.blocks`` operator surface.
 
 ``import bifrost_b200 as bf`` exposes the subset of ``import bifrost as bf``

@@ -91,6 +91,10 @@ class SigprocSinkBlock(SinkBlock):
         hdr = {}
         for key in ('source_name', 'rawdatafile', 'az_start', 'za_start'):
             _copy_item_if_exists(hdr, ihdr, key)
+        if 'rawdatafile' in hdr:
+            # the GUPPI reader passes the path it read; sigproc strings hold at
+            # most 79 bytes, so the card keeps the file name
+            hdr['rawdatafile'] = os.path.basename(str(hdr['rawdatafile']))
         _copy_item_if_exists(hdr, ihdr, 'raj', 'src_raj')
         _copy_item_if_exists(hdr, ihdr, 'dej', 'src_dej')
         if ihdr.get('telescope') is not None:

@@ -1,4 +1,4 @@
-"""spectrometer block: the fused GUPPI chain as one block (B200 extension).
+"""spectrometer block: the fused GUPPI chain as one block (extension).
 
     b = bf.blocks.spectrometer(copy_to_cuda_block, f_avg=4, n_int=8)
 

@@ -1,4 +1,4 @@
-// fdmt.cu -- bfFdmt* for sm_100a.
+// fdmt.cu -- bfFdmt* for sm_90a.
 //
 // Replaces: src/fdmt.cu:724-814 (C entry points), :531-628 (storage
 // protocol), :629-718 (execute), :52-92 (init kernel), :95-155 (step kernel).
@@ -139,7 +139,8 @@ fdmt_step_kernel(const float* __restrict__ prev, long pstride, long pbatchstride
 //  * TAIL (steps K+1..last): the wide, few-band steps cannot fit on chip; they
 //    run as row-blocked step kernels (adjacent output rows share source rows,
 //    so a CTA's re-reads hit L1) swept tile-by-tile over time so that the
-//    ping-pong working set of all tail steps stays in the 126 MB L2.
+//    ping-pong working set of all tail steps stays in L2 (50 MB on H100;
+//    BFB_FDMT_TAIL_TILE sets the tile).
 // Every value is produced by exactly the fp32 operations of the reference
 // (explicit __fadd_rn/__fmul_rn: no FMA contraction across the step-0 scale
 // and the level-1 add), so v2 is bit-identical to v1 and to the reference.
@@ -743,15 +744,15 @@ static bool build_packed_passes(FdmtPlan const& P, std::vector<std::vector<char>
 		PackedCfg cfg;
 		const size_t pi = passes.size();
 		cfg.D       = pi < Ds.size()  ? Ds[pi]  : (s0 == 1 ? 64 : 24);
-		// 8 warps (three CTAs per SM) for the pass that reads the 1-byte input, 12 (two
-		// CTAs per SM, 24 warps) for the others -- measured: 0.866 vs 0.877 ms with 8
+		// 8 warps for every pass.  Four CTAs per SM for the pass that reads the 1-byte
+		// input (its source shares region 0 with the merged rows: 54 KB per CTA, 64
+		// registers), three for the others (72 KB each).  Chosen on an H100 (SXM,
+		// 700 W) over 12 / 16 warps and 110 / 150 KB for the later passes: config 2
+		// with max_delay 204 / 794 / 1621 took 0.59 / 1.46 / 3.33 ms, against
+		// 0.62 / 1.56 / 3.56 ms with 12 warps and 110 KB (all with 16 waves below).
 		const bool nw8 = (s0 == 1 || (pi < LVs.size() && LVs[pi] == 5)) || env_int("BFB_FDMT_PACKED_MEGA", 0) != 0;   // (the persistent kernel runs 8 warps)
-		cfg.nwarp   = std::max(1, std::min(nw8 ? 8 : 16, pi < NWs.size() ? NWs[pi] : (nw8 ? 8 : 12)));
-		// four CTAs per SM for the pass that reads the 1-byte input (its source shares
-		// region 0 with the merged rows: 54 KB per CTA, 64 registers), two -- larger
-		// delay blocks, fewer redundant rows -- for the others: measured optimum for
-		// config 2 (0.83 ms; with a source region of its own and three CTAs: 0.87)
-		cfg.smem_cap = 1024 * std::min(227, pi < SMs.size() ? SMs[pi] : (s0 == 1 ? 56 : 110));
+		cfg.nwarp   = std::max(1, std::min(nw8 ? 8 : 16, pi < NWs.size() ? NWs[pi] : 8));
+		cfg.smem_cap = 1024 * std::min(227, pi < SMs.size() ? SMs[pi] : (s0 == 1 ? 56 : 72));
 		cfg.tcap    = pi < TCs.size() ? std::max(64, TCs[pi]) : (1 << 20);
 		cfg.fuse4   = env_int("BFB_FDMT_PACKED_FUSE", 1) != 0;
 		cfg.own_src = pi < PFs.size() ? PFs[pi] != 0 : false;        // (a region of its own for the source: opt-in)
@@ -892,14 +893,15 @@ static BFstatus launch_packed_pass(PackedPass const& cp, PackedParams const& q, 
 	if( nprog == 0 ) return BF_STATUS_SUCCESS;
 	// CTAs walk their program's tiles with a stride: about `waves` launch waves
 	// of 2 CTAs per SM in total, so the op tables are copied to shared memory a
-	// few times per program instead of once per tile.
+	// few times per program instead of once per tile (16 waves: about 4 % faster
+	// than 8 for config 2 on an H100).
 	static int sm_count = 0;
 	if( !sm_count ) {
 		int dev = 0;
 		cudaGetDevice(&dev);
-		if( cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0 ) sm_count = 148;
+		if( cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0 ) sm_count = 132;
 	}
-	const long waves = std::max(1, env_int("BFB_FDMT_PACKED_WAVES", 8));
+	const long waves = std::max(1, env_int("BFB_FDMT_PACKED_WAVES", 16));
 	long gx = div_up<long>(2L * sm_count * waves, (long)nprog * nbatch);
 	gx = std::max<long>(1, std::min<long>(gx, q.ntile));
 	gx = div_up<long>(q.ntile, div_up<long>(q.ntile, gx));      // equal shares
@@ -1257,7 +1259,7 @@ BFstatus bfFdmtTileQuery(BFsize nchan, BFsize max_delay, double f0, double df,
 }
 
 // ---------------------------------------------------------------------------
-// Sharded execution (B200 extension; SURVEY 8f.1, DESIGN 6): the FULL-BAND
+// Sharded execution (extension; SURVEY 8f.1, DESIGN 6): the FULL-BAND
 // transform over `nrank` cooperating plans, one per GPU.  Every rank calls
 // bfFdmtInit with the same (full-band) arguments and then bfFdmtShardInit.
 // The merge tree has `nrank` sub-bands at the split step; rank g owns the
@@ -1385,10 +1387,9 @@ BFstatus bfFdmtShardExecutePeers(BFfdmt plan, BFarray const* in, BFarray const* 
 	PackedPass const& sp = plan->packed[plan->shard_split];
 	PackedPeers peers;
 	peers.n = npeer; peers.self = plan->shard_rank;
-	// remote rows: plain 16-byte loads by all warps (measured on 2 B200s, config 2's
-	// gulp: 0.84 ms per gulp); BFB_FDMT_PEER_TMA=1 stages them with cp.async.bulk
-	// like the local ones (works, 0.99 ms: a bulk copy over NVLink completes late
-	// and the tile waits for the slowest one)
+	// remote rows: plain 16-byte loads by all warps; BFB_FDMT_PEER_TMA=1 stages
+	// them with cp.async.bulk like the local ones (a bulk copy over NVLink
+	// completes late and the tile waits for the slowest one)
 	peers.ldg = env_int("BFB_FDMT_PEER_TMA", 0) ? 0 : 1;
 	for( int g=0; g<=npeer; ++g ) {
 		const int r0 = g < npeer ? P.bands[plan->shard_step][g].row0 : P.nrow(plan->shard_step);

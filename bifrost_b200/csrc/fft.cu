@@ -1,4 +1,4 @@
-// fft.cu -- bfFft* for sm_100a, hand-written (no cuFFT).
+// fft.cu -- bfFft* for sm_90a, hand-written (no cuFFT).
 //
 // Replaces: src/fft.cu:109-419 (plan + execute over cufftMakePlanMany64) and
 // src/fft_kernels.cu:32-341 (load callbacks: integer -> float scaling and

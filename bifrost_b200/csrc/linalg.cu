@@ -1,4 +1,4 @@
-// linalg.cu -- bfLinAlg* for sm_100a: the cross-correlation ("X-engine") call
+// linalg.cu -- bfLinAlg* for sm_90a: the cross-correlation ("X-engine") call
 // behind bf.blocks.correlate.
 //
 // Replaces: src/linalg.cu:877-904 (bfLinAlgMatMul), :242-357 (bfMatMul_aa),
@@ -12,19 +12,18 @@
 // test/test_linalg.py:168-185).  Integer inputs accumulate exactly in int32.
 //
 // Two kernels:
-//  * corr_tc_kernel -- tcgen05 int8 tensor cores.  The interleaved complex
+//  * corr_tc_kernel -- int8 wgmma tensor cores.  The interleaved complex
 //    samples of one frequency channel form a real row-major matrix
 //    M[t][2i+p] (p = re/im).  Its Gram matrix G = M^T M holds all four real
 //    products of every pair: Re C_ij = G[2i][2j] + G[2i+1][2j+1],
 //    Im C_ij = G[2i][2j+1] - G[2i+1][2j].  Time (the reduction dim) is the slow
 //    axis in memory, i.e. both MMA operands are MN-major: TMA drops
-//    [64 t][128 B] boxes with the 128-byte swizzle straight into the canonical
-//    MN-major UMMA layout, one elected thread issues
-//    tcgen05.mma.kind::i8 (M=128, N=128, K=32) into a TMEM accumulator, and four
-//    epilogue warps pull the int32 tile out of TMEM, pair rows with a lane
-//    shuffle, and write the lower-triangular cf32 tile through shared memory
-//    so that global stores are row-contiguous.  Only tiles on or below the
-//    diagonal are launched; diagonal tiles load one operand.
+//    [64 t][128 B] boxes into a stage ring, the two consumer warpgroups
+//    transpose them in shared memory into the K-major layout int8 wgmma reads,
+//    issue wgmma.m64n128k32.s32.s8.s8 into register accumulators, pair rows
+//    with a lane shuffle, and write the lower-triangular cf32 tile through
+//    shared memory so that global stores are row-contiguous.  Only tiles on or
+//    below the diagonal are launched; diagonal tiles load one operand.
 //  * corr_simt_kernel -- shared-memory tiled SIMT fallback for layouts TMA
 //    cannot describe (strides not multiples of 16 B, a.a^H form, ci16/cf32).
 #include "core.hpp"
@@ -120,9 +119,19 @@ corr_simt_kernel(SimtParams P) {
 		}
 }
 
-// ============================================================ tcgen05 kernel
-enum { TC_KT = 64, TC2_STAGES = 3, TC_TILE_BYTES = TC_KT * 128, TC_THREADS = 192,
-       TC_STAGE_BYTES = 3 * TC_TILE_BYTES };    // A | B0 | B1
+// ============================================================ wgmma kernels
+// One CTA computes a 128 x (128 or 256) int32 tile of a real Gram-type product
+// G = A^T B, where A and B are MN-major int8 matrices (the reduction dim is the
+// slow axis in memory).  Warp 8 is the TMA producer: [64 k][128 B] boxes land
+// in a TC_STAGES-deep ring of raw stages.  Warps 0..7 (two warpgroups) are the
+// consumers: int8 wgmma reads K-major operands only, so each stage is first
+// transposed in shared memory (4x4 byte blocks, PRMT) into the no-swizzle
+// K-major core-matrix layout, then warpgroup g issues
+// wgmma.m64n128k32.s32.s8.s8 for rows 64 g .. 64 g + 63 of the tile.  The
+// K-major buffer is double-buffered so that the transpose of slab k+1 overlaps
+// the MMAs of slab k.
+enum { TC_KT = 64, TC_STAGES = 3, TC_TILE_BYTES = TC_KT * 128, TC_CONSUMERS = 256,
+       TC_THREADS = TC_CONSUMERS + 32, TC_STAGE_BYTES = 3 * TC_TILE_BYTES };   // A | B0 | B1
 
 struct TcParams {
 	float2* c; long c_row, c_batch;      // float2 units
@@ -142,6 +151,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 	asm volatile(
 		"{\n\t.reg .pred p;\n\t"
@@ -159,79 +171,208 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 		" [%0], [%1, {%3, %4, %5}], [%2];"
 		:: "r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z) : "memory");
 }
-// 64-bit shared-memory matrix descriptor: MN-major, 128-byte swizzle, one
-// 128-byte atom wide; 8-row groups are 1024 B apart (SBO).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr) {
+
+// wgmma shared-memory descriptor of a K-major operand without swizzle: 8-row x
+// 16-byte core matrices of 128 contiguous bytes; the next core matrix along K
+// is 128 B on (leading byte offset), the next 8-row group 512 B (stride byte
+// offset) -- a 64-byte K slab per row (TC_KT int8).
+__device__ __forceinline__ uint64_t gmma_desc_k_inter(uint32_t saddr) {
 	uint64_t d = 0;
-	d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address
-	d |= (uint64_t)(TC_TILE_BYTES >> 4) << 16;        // leading byte offset: next 128-byte atom along MN (N = 256)
-	d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset between 8-row groups
-	d |= (uint64_t)1 << 46;                           // descriptor version (Blackwell)
-	d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
-	return d;
-}
-// Instruction descriptor: S32 accumulate, signed int8 A and B, both MN-major,
-// M = 128, N = 128 or 256.
-__device__ __forceinline__ uint32_t umma_idesc_i8(uint32_t n_dim) {
-	uint32_t d = 0;
-	d |= 2u << 4;            // c_format = S32
-	d |= 1u << 7;            // a_format = INT8 (signed)
-	d |= 1u << 10;           // b_format = INT8 (signed)
-	d |= 1u << 15;           // a_major = MN
-	d |= 1u << 16;           // b_major = MN
-	d |= (n_dim >> 3) << 17; // n_dim
-	d |= (128u >> 4) << 24;  // m_dim
-	return d;
+	d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+	d |= (uint64_t)(128 >> 4) << 16;
+	d |= (uint64_t)(512 >> 4) << 32;
+	return d;                                          // layout type 0: no swizzle
 }
 
-// Epilogue of one (row block I, column blocks J0 .. J0+nb-1) unit, run by warps
-// 2..5: TMEM -> registers (32x32b.x32), combine the interleaved re/im rows of
-// the real Gram matrix into complex visibilities with a lane-pair shuffle,
-// stage through shared memory and store coalesced lower-triangle cf32.
-__device__ __forceinline__ void tc_epilogue(uint64_t* tmem_bar, uint32_t tmem_base, float2* staging,
-                                            TcParams const& P, int batch, int I, int J0, int nb,
-                                            int warp, int lane) {
-	mbar_wait(tmem_bar, 0);
-	asm volatile("tcgen05.fence::after_thread_sync;");
-	const int quarter = warp & 3;                       // TMEM lane quarter this warp may read
-	const int m = quarter * 32 + lane;                  // row of the 128 x 256 int32 tile
-	const int il = m >> 1, par = m & 1;                 // complex row, re/im row of the pair
-	float* stf = (float*)staging;
-	const int te = threadIdx.x - 64;                    // 0..127
-	float2* cb = P.c + (long)batch * P.c_batch;
-	for( int h=0; h<nb; ++h ) {
-		const int J = J0 + h;
-#pragma unroll 1
-		for( int c0=0; c0<128; c0+=32 ) {
-			uint32_t r[32];
-			const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(128 * h + c0);
-			asm volatile(
-				"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-				"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-				"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-				: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-				  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-				  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-				  "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-				: "r"(taddr));
-			asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Raw TMA tile raw[k][r] (64 x 128 bytes) -> K-major kt: row r, byte k at
+// ((r/8)*4 + k/16)*128 + (r%8)*16 + k%16.  Each consumer thread moves two 4x4
+// byte blocks; the lane mapping keeps both the loads and the stores at 4-way
+// bank conflicts at most.
+__device__ __forceinline__ void tc_transpose(const unsigned char* raw, unsigned char* kt, int tid) {
+	const int l = tid & 31, wq = tid >> 5;
+	const uint32_t* src = (const uint32_t*)raw;
 #pragma unroll
-			for( int q=0; q<16; ++q ) {
-				// even row 2i holds (G[2i][2j], G[2i][2j+1]); odd row holds
-				// (G[2i+1][2j], G[2i+1][2j+1]); swap the second entries.
-				int mine0 = (int)r[2*q], mine1 = (int)r[2*q+1];
-				int other1 = __shfl_xor_sync(0xffffffffu, mine1, 1);
-				// even lane: Re = G[2i][2j] + G[2i+1][2j+1]; odd lane: Im = G[2i][2j+1] - G[2i+1][2j]
-				int v = par ? (other1 - mine0) : (mine0 + other1);
-				int jl = (c0 >> 1) + q;
-				stf[(il * 65 + jl) * 2 + par] = (float)v;
+	for( int k=0; k<2; ++k ) {
+		const int r4 = (l & 1) | (((l >> 3) & 3) << 1) | ((wq & 3) << 3);
+		const int t4 = ((l >> 1) & 3) | (((wq >> 2) & 1) << 2) | (k << 3);
+		const uint32_t w0 = src[(4 * t4 + 0) * 32 + r4], w1 = src[(4 * t4 + 1) * 32 + r4];
+		const uint32_t w2 = src[(4 * t4 + 2) * 32 + r4], w3 = src[(4 * t4 + 3) * 32 + r4];
+		const uint32_t a = __byte_perm(w0, w1, 0x5140), b = __byte_perm(w0, w1, 0x7362);
+		const uint32_t c = __byte_perm(w2, w3, 0x5140), d = __byte_perm(w2, w3, 0x7362);
+		const uint32_t o[4] = { __byte_perm(a, c, 0x5410), __byte_perm(a, c, 0x7632),
+		                        __byte_perm(b, d, 0x5410), __byte_perm(b, d, 0x7632) };
+		const int t = 4 * t4;
+#pragma unroll
+		for( int j=0; j<4; ++j ) {
+			const int r = 4 * r4 + j;
+			*(uint32_t*)(kt + ((r >> 3) * 4 + (t >> 4)) * 128 + (r & 7) * 16 + (t & 15)) = o[j];
+		}
+	}
+}
+
+// d = A(64 x 32) . B(32 x 128) + (accumulate ? d : 0), both operands from shared memory
+__device__ __forceinline__ void wgmma_m64n128k32_s8(int (&d)[64], uint64_t da, uint64_t db, int accumulate) {
+	asm volatile(
+		"{\n\t.reg .pred p;\n\t"
+		"setp.ne.b32 p, %66, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+		"%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+		"%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+		"%64, %65, p;\n\t}"
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+		  "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+		  "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+		  "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+		  "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+		  "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+		  "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+		  "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+		: "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+
+// Shared-memory layout of both kernels:
+//   [TC_STAGES raw stages | 2 K-major buffers] of TC_STAGE_BYTES each,
+//   staging float2[64][65], full / empty barriers.
+__host__ __device__ constexpr size_t tc_smem_bytes() {
+	return (size_t)(TC_STAGES + 2) * TC_STAGE_BYTES + 64 * 65 * sizeof(float2) +
+	       2 * TC_STAGES * sizeof(uint64_t) + 1024;          // + 1024: alignment of the window
+}
+
+// Main loop of one work unit: G rows 128 I' .. (A operand, x coordinate ax,
+// batch az) times nb column blocks of 128 (B operand from bx0, batch bz).
+// alias = 1 / 2: A is the same block as B0 / B1 and is not loaded.  Returns in
+// acc[h] the warpgroup's 64 x 128 int32 fragment of column block h (consumer
+// threads only; the producer warp returns false).
+__device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtensorMap* ta, const CUtensorMap* tb,
+                                            int ax, int az, int bx0, int bz, int nb, int alias, int nk,
+                                            int (&acc)[2][64]) {
+	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
+	unsigned char* ktbuf = tiles + TC_STAGES * TC_STAGE_BYTES;
+	float2* staging = (float2*)(ktbuf + 2 * TC_STAGE_BYTES);
+	uint64_t* full_bar  = (uint64_t*)(staging + 64 * 65);
+	uint64_t* empty_bar = full_bar + TC_STAGES;
+	const int tid = threadIdx.x;
+
+	if( tid == 0 ) {
+		for( int s=0; s<TC_STAGES; ++s ) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], TC_CONSUMERS); }
+		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+	}
+	__syncthreads();
+
+	if( tid >= TC_CONSUMERS ) {
+		// ===================== TMA producer =====================
+		if( tid == TC_CONSUMERS ) {
+			const uint32_t bytes = (uint32_t)TC_TILE_BYTES * (nb + (alias ? 0 : 1));
+			for( int it=0; it<nk; ++it ) {
+				const int s = it % TC_STAGES;
+				const uint32_t ph = (it / TC_STAGES) & 1;
+				mbar_wait(&empty_bar[s], ph ^ 1);
+				unsigned char* a = tiles + (size_t)s * TC_STAGE_BYTES;
+				mbar_expect_tx(&full_bar[s], bytes);
+				if( !alias ) tma_load_3d(a, ta, &full_bar[s], ax, it * TC_KT, az);
+				tma_load_3d(a + TC_TILE_BYTES, tb, &full_bar[s], bx0, it * TC_KT, bz);
+				if( nb == 2 ) tma_load_3d(a + 2 * TC_TILE_BYTES, tb, &full_bar[s], bx0 + 128, it * TC_KT, bz);
 			}
 		}
-		// all four epilogue warps have staged their rows
-		asm volatile("bar.sync 1, 128;" ::: "memory");
-		for( int idx = te; idx < 64 * 64; idx += 128 ) {
-			int il2 = idx >> 6, jl2 = idx & 63;
-			int i = I * 64 + il2, j = J * 64 + jl2;
+		return false;
+	}
+
+	// ===================== consumers: transpose + wgmma =====================
+	const int wg = tid >> 7;
+	for( int it=0; it<nk; ++it ) {
+		const int s = it % TC_STAGES;
+		const uint32_t ph = (it / TC_STAGES) & 1;
+		mbar_wait(&full_bar[s], ph);
+		const unsigned char* raw = tiles + (size_t)s * TC_STAGE_BYTES;
+		unsigned char* kt = ktbuf + (size_t)(it & 1) * TC_STAGE_BYTES;
+		if( !alias ) tc_transpose(raw, kt, tid);
+		tc_transpose(raw + TC_TILE_BYTES, kt + TC_TILE_BYTES, tid);
+		if( nb == 2 ) tc_transpose(raw + 2 * TC_TILE_BYTES, kt + 2 * TC_TILE_BYTES, tid);
+		// the K-major writes are read by the async proxy (wgmma)
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+		mbar_arrive(&empty_bar[s]);
+		// this warpgroup's MMAs of the previous slab have finished reading the
+		// other K-major buffer, and every consumer's transpose of this slab is done
+		asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
+		asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+		const uint32_t kt_addr = smem_u32(kt);
+		const uint32_t b_addr = kt_addr + TC_TILE_BYTES;
+		const uint32_t a_addr = (alias == 1 ? b_addr : alias == 2 ? b_addr + TC_TILE_BYTES : kt_addr) + wg * 4096;
+#pragma unroll
+		for( int kk=0; kk<TC_KT/32; ++kk ) {
+			const uint64_t da = gmma_desc_k_inter(a_addr + kk * 256);
+			const int accumulate = (it > 0 || kk > 0) ? 1 : 0;          // the first MMA zeroes the tile
+			wgmma_m64n128k32_s8(acc[0], da, gmma_desc_k_inter(b_addr + kk * 256), accumulate);
+			if( nb == 2 ) wgmma_m64n128k32_s8(acc[1], da, gmma_desc_k_inter(b_addr + TC_TILE_BYTES + kk * 256), accumulate);
+		}
+		asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+	}
+	asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+	// the accumulators are final only now: keep their reads below the wait
+#pragma unroll
+	for( int h=0; h<2; ++h )
+#pragma unroll
+		for( int q=0; q<64; ++q ) asm volatile("" : "+r"(acc[h][q]) :: "memory");
+	return true;
+}
+
+// Fragment of column block h -> staging[64][65] (complex rows il, columns jl).
+// The wgmma accumulator holds, per thread, rows 64 g + 16 w + lane/4 (+8) and
+// column pairs (c, c+1), c = 8 j + 2 (lane%4): even rows 2i carry (G[2i][2j],
+// G[2i][2j+1]), odd rows (G[2i+1][2j], G[2i+1][2j+1]), in lanes 4 apart.
+// combine(mine0, other1, par) makes the real (par 0) or imaginary part.
+template<typename F>
+__device__ __forceinline__ void tc_stage(int const (&acc)[64], float2* staging, F combine) {
+	const int tid = threadIdx.x, lane = tid & 31;
+	const int row0 = 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + (lane >> 2);
+	const int par = row0 & 1;
+	float* stf = (float*)staging;
+#pragma unroll
+	for( int j=0; j<16; ++j )
+#pragma unroll
+		for( int hf=0; hf<2; ++hf ) {
+			const int mine0 = acc[4 * j + 2 * hf], mine1 = acc[4 * j + 2 * hf + 1];
+			const int other1 = __shfl_xor_sync(0xffffffffu, mine1, 4);
+			const int il = (row0 + 8 * hf) >> 1, jl = 4 * j + (lane & 3);
+			stf[(il * 65 + jl) * 2 + par] = combine(mine0, other1, par);
+		}
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	const int batch = blockIdx.y;
+	// Work unit: row block I (128 rows of the real Gram matrix) x a pair of
+	// column blocks (2 JJ, 2 JJ + 1) with 2 JJ <= I.  The second block is
+	// dropped when it lies above the diagonal (nb = 1).  A 128 x 256 tile moves
+	// 24 KB per K slab for two blocks instead of 32 KB (DESIGN.md §4).
+	int I = 0, rem = blockIdx.x;
+	while( rem >= I / 2 + 1 ) { rem -= I / 2 + 1; ++I; }
+	const int J0 = 2 * rem;
+	const int nb = (J0 + 1 <= I) ? 2 : 1;
+	// operand aliasing: a column block equal to the row block is loaded once
+	const int alias = (J0 == I) ? 1 : (nb == 2 && J0 + 1 == I) ? 2 : 0;
+	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
+	int acc[2][64];
+	if( !tc_mainloop(tc_smem, &tmap, &tmap, 128 * I, batch, 128 * J0, batch, nb, alias, nk, acc) ) return;
+
+	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
+	float2* staging = (float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
+	float2* cb = P.c + (long)batch * P.c_batch;
+#pragma unroll
+	for( int h=0; h<2; ++h ) {
+		if( h >= nb ) break;
+		const int J = J0 + h;
+		// even lane: Re = G[2i][2j] + G[2i+1][2j+1]; odd lane: Im = G[2i][2j+1] - G[2i+1][2j]
+		tc_stage(acc[h], staging, [](int mine0, int other1, int par) {
+			return (float)(par ? (other1 - mine0) : (mine0 + other1)); });
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
+		for( int idx = threadIdx.x; idx < 64 * 64; idx += TC_CONSUMERS ) {
+			const int il2 = idx >> 6, jl2 = idx & 63;
+			const int i = I * 64 + il2, j = J * 64 + jl2;
 			if( i < P.n && j < P.n && i >= j ) {
 				float2 v = staging[il2 * 65 + jl2];
 				if( P.conj_u ) v.y = -v.y;
@@ -242,241 +383,8 @@ __device__ __forceinline__ void tc_epilogue(uint64_t* tmem_bar, uint32_t tmem_ba
 			}
 		}
 		// the staging buffer is reused by the second column block
-		asm volatile("bar.sync 1, 128;" ::: "memory");
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
 	}
-	}
-
-template<int TC_STAGES>
-__global__ void __launch_bounds__(TC_THREADS)
-corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
-	extern __shared__ __align__(1024) unsigned char tc_smem[];
-	// layout: [stages][A 8 KB | B0 8 KB | B1 8 KB] | staging float2[64][65] | barriers
-	// the swizzled operand tiles need 1024-byte alignment in the shared window
-	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
-	float2* staging = (float2*)(tiles + TC_STAGES * TC_STAGE_BYTES);
-	uint64_t* full_bar  = (uint64_t*)(staging + 64 * 65);
-	uint64_t* empty_bar = full_bar + TC_STAGES;
-	uint64_t* tmem_bar  = empty_bar + TC_STAGES;
-	uint32_t* tmem_slot = (uint32_t*)(tmem_bar + 1);
-
-	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const int batch = blockIdx.y;
-	// Work unit: row block I (128 rows of the real Gram matrix) x a pair of
-	// column blocks (2 JJ, 2 JJ + 1) with 2 JJ <= I.  The second block is
-	// dropped when it lies above the diagonal (nb = 1).  A 128 x 256 tile moves
-	// 24 KB per K slab for two blocks instead of 32 KB: the kernel is bound by
-	// L2 -> SM operand traffic, not by the tensor pipe (DESIGN.md 4.7).
-	int I = 0, rem = blockIdx.x;
-	while( rem >= I / 2 + 1 ) { rem -= I / 2 + 1; ++I; }
-	const int J0 = 2 * rem;
-	const int nb = (J0 + 1 <= I) ? 2 : 1;
-	// operand aliasing: a column block equal to the row block is loaded once
-	const bool a_is_b0 = (J0 == I), a_is_b1 = (nb == 2 && J0 + 1 == I);
-	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
-
-	if( threadIdx.x == 0 ) {
-		for( int s=0; s<TC_STAGES; ++s ) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-		mbar_init(tmem_bar, 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	if( warp == 1 ) {
-		// 256 TMEM columns: a 128 x 256 int32 accumulator; the address lands in smem
-		asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-		             :: "r"(smem_u32(tmem_slot)), "n"(256));
-		asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	asm volatile("tcgen05.fence::after_thread_sync;");
-	const uint32_t tmem_base = *tmem_slot;
-
-	if( warp == 0 ) {
-		// ===================== TMA producer =====================
-		if( lane == 0 ) {
-			const uint32_t bytes = (uint32_t)TC_TILE_BYTES * (nb + ((a_is_b0 || a_is_b1) ? 0 : 1));
-			for( int it=0; it<nk; ++it ) {
-				const int s = it % TC_STAGES;
-				const uint32_t ph = (it / TC_STAGES) & 1;
-				mbar_wait(&empty_bar[s], ph ^ 1);
-				unsigned char* a = tiles + (size_t)s * TC_STAGE_BYTES;
-				mbar_expect_tx(&full_bar[s], bytes);
-				if( !(a_is_b0 || a_is_b1) ) tma_load_3d(a, &tmap, &full_bar[s], 128 * I, it * TC_KT, batch);
-				tma_load_3d(a + TC_TILE_BYTES, &tmap, &full_bar[s], 128 * J0, it * TC_KT, batch);
-				if( nb == 2 ) tma_load_3d(a + 2 * TC_TILE_BYTES, &tmap, &full_bar[s], 128 * (J0 + 1), it * TC_KT, batch);
-			}
-		}
-	} else if( warp == 1 ) {
-		// ===================== MMA issuer =====================
-		const uint32_t idesc = umma_idesc_i8(nb == 2 ? 256u : 128u);
-		for( int it=0; it<nk; ++it ) {
-			const int s = it % TC_STAGES;
-			const uint32_t ph = (it / TC_STAGES) & 1;
-			mbar_wait(&full_bar[s], ph);
-			asm volatile("tcgen05.fence::after_thread_sync;");
-			if( lane == 0 ) {
-				const uint32_t st_addr = smem_u32(tiles + (size_t)s * TC_STAGE_BYTES);
-				const uint32_t b_addr = st_addr + TC_TILE_BYTES;
-				const uint32_t a_addr = a_is_b0 ? b_addr : (a_is_b1 ? b_addr + TC_TILE_BYTES : st_addr);
-#pragma unroll
-				for( int kk=0; kk<TC_KT/32; ++kk ) {
-					const uint64_t da = umma_desc_mn_sw128(a_addr + kk * 32 * 128);
-					const uint64_t db = umma_desc_mn_sw128(b_addr + kk * 32 * 128);
-					const uint32_t acc = (it > 0 || kk > 0) ? 1u : 0u;
-					asm volatile(
-						"{\n\t.reg .pred p;\n\t"
-						"setp.ne.b32 p, %4, 0;\n\t"
-						"tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-						:: "r"(tmem_base), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-				}
-				// release the smem stage once these MMAs have consumed it
-				asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-				             :: "r"(smem_u32(&empty_bar[s])) : "memory");
-				if( it == nk - 1 ) {
-					asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-					             :: "r"(smem_u32(tmem_bar)) : "memory");
-				}
-			}
-			__syncwarp();
-		}
-	} else {
-		tc_epilogue(tmem_bar, tmem_base, staging, P, batch, I, J0, nb, warp, lane);
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	if( warp == 1 ) {
-		asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(256));
-	}
-}
-
-// ---------------------------------------------------------------------------
-// Cluster variant: a CTA pair owns the 256 x 256 super tile (row blocks 2 II
-// and 2 II + 1) x (column blocks 2 JJ and 2 JJ + 1), JJ <= II.  Each CTA loads
-// ONE of the two column blocks per K slab and TMA-multicasts it to both CTAs, so
-// the pair moves A0 + A1 + B0 + B1 = 32 KB per slab for four output blocks
-// (8 KB per block instead of 12).  On diagonal super tiles the row blocks ARE
-// the column blocks and nothing else is loaded.  A stage may be refilled only
-// after BOTH CTAs' MMAs have released it: every tcgen05.commit is multicast to
-// the empty barrier of both CTAs (count 2).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-	uint32_t r;
-	asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-	return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-	asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-	asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* map, uint64_t* bar,
-                                               int x, int y, int z, uint16_t mask) {
-	asm volatile(
-		"cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-		" [%0], [%1, {%3, %4, %5}], [%2], %6;"
-		:: "r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z), "h"(mask) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS)
-corr_tc2_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
-	extern __shared__ __align__(1024) unsigned char tc_smem[];
-	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
-	float2* staging = (float2*)(tiles + TC2_STAGES * TC_STAGE_BYTES);
-	uint64_t* full_bar  = (uint64_t*)(staging + 64 * 65);
-	uint64_t* empty_bar = full_bar + TC2_STAGES;
-	uint64_t* tmem_bar  = empty_bar + TC2_STAGES;
-	uint32_t* tmem_slot = (uint32_t*)(tmem_bar + 1);
-
-	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const int batch = blockIdx.y;
-	const int rank = (int)cluster_ctarank();            // 0 / 1: upper / lower row block of the pair
-	// super tile index -> (II, JJ), II >= JJ
-	const int st = blockIdx.x >> 1;
-	int II = (int)((sqrtf(8.f * st + 1.f) - 1.f) * 0.5f);
-	while( II * (II + 1) / 2 > st ) --II;
-	while( (II + 1) * (II + 2) / 2 <= st ) ++II;
-	const int JJ = st - II * (II + 1) / 2;
-	const bool sdiag = (II == JJ);
-	const int I = 2 * II + rank, J0 = 2 * JJ;
-	// column blocks this CTA needs: on the diagonal super tile the upper row
-	// block only has its own diagonal block
-	const int nb = (sdiag && rank == 0) ? 1 : 2;
-	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
-
-	if( threadIdx.x == 0 ) {
-		for( int s=0; s<TC2_STAGES; ++s ) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
-		mbar_init(tmem_bar, 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	if( warp == 1 ) {
-		asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-		             :: "r"(smem_u32(tmem_slot)), "n"(256));
-		asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	asm volatile("tcgen05.fence::after_thread_sync;");
-	const uint32_t tmem_base = *tmem_slot;
-	// the peer's barriers must be initialised before anything is multicast to it
-	cluster_sync_all();
-
-	if( warp == 0 ) {
-		// ===================== TMA producer =====================
-		if( lane == 0 ) {
-			// both column blocks always arrive (one from each CTA); the row block
-			// is loaded only off the diagonal
-			const uint32_t bytes = (uint32_t)TC_TILE_BYTES * (sdiag ? 2 : 3);
-			for( int it=0; it<nk; ++it ) {
-				const int s = it % TC2_STAGES;
-				const uint32_t ph = (it / TC2_STAGES) & 1;
-				mbar_wait(&empty_bar[s], ph ^ 1);            // both CTAs have released the stage
-				unsigned char* a = tiles + (size_t)s * TC_STAGE_BYTES;
-				mbar_expect_tx(&full_bar[s], bytes);
-				if( !sdiag ) tma_load_3d(a, &tmap, &full_bar[s], 128 * I, it * TC_KT, batch);
-				tma_load_3d_mc(a + (1 + rank) * TC_TILE_BYTES, &tmap, &full_bar[s],
-				               128 * (J0 + rank), it * TC_KT, batch, (uint16_t)0x3);
-			}
-		}
-	} else if( warp == 1 ) {
-		// ===================== MMA issuer =====================
-		const uint32_t idesc = umma_idesc_i8(nb == 2 ? 256u : 128u);
-		for( int it=0; it<nk; ++it ) {
-			const int s = it % TC2_STAGES;
-			const uint32_t ph = (it / TC2_STAGES) & 1;
-			mbar_wait(&full_bar[s], ph);
-			asm volatile("tcgen05.fence::after_thread_sync;");
-			if( lane == 0 ) {
-				const uint32_t st_addr = smem_u32(tiles + (size_t)s * TC_STAGE_BYTES);
-				const uint32_t b_addr = st_addr + TC_TILE_BYTES;
-				const uint32_t a_addr = sdiag ? b_addr + rank * TC_TILE_BYTES : st_addr;
-#pragma unroll
-				for( int kk=0; kk<TC_KT/32; ++kk ) {
-					const uint64_t da = umma_desc_mn_sw128(a_addr + kk * 32 * 128);
-					const uint64_t db = umma_desc_mn_sw128(b_addr + kk * 32 * 128);
-					const uint32_t acc = (it > 0 || kk > 0) ? 1u : 0u;
-					asm volatile(
-						"{\n\t.reg .pred p;\n\t"
-						"setp.ne.b32 p, %4, 0;\n\t"
-						"tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-						:: "r"(tmem_base), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-				}
-				// release the stage in BOTH CTAs once these MMAs have consumed it
-				asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-				             :: "r"(smem_u32(&empty_bar[s])), "h"((uint16_t)0x3) : "memory");
-				if( it == nk - 1 ) {
-					asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-					             :: "r"(smem_u32(tmem_bar)) : "memory");
-				}
-			}
-			__syncwarp();
-		}
-	} else {
-		tc_epilogue(tmem_bar, tmem_base, staging, P, batch, I, J0, nb, warp, lane);
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	if( warp == 1 ) {
-		asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(256));
-	}
-	// neither CTA may exit while the other can still multicast into it
-	cluster_sync_all();
 }
 
 // ---------------------------------------------------------------------------
@@ -488,8 +396,8 @@ corr_tc2_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 // int8 product G = At^T B holds the four real products of every (m, n):
 //   Re c = G[2m][2n] - G[2m+1][2n+1],   Im c = G[2m][2n+1] + G[2m+1][2n]
 // (signs flip with the operands' conjugation flags).  Both operands are
-// MN-major exactly like the correlator's, so TMA boxes, UMMA descriptors, the
-// stage pipeline and the TMEM epilogue are shared; the sums are exact integers.
+// MN-major exactly like the correlator's, so TMA boxes, the stage pipeline,
+// the transpose and the wgmma main loop are shared; the sums are exact integers.
 // A work unit is a 128 x 256 tile of G = 64 x 128 complex outputs.
 // ---------------------------------------------------------------------------
 struct AbTcParams {
@@ -501,46 +409,30 @@ struct AbTcParams {
 	float s_re, s_01, s_10;              // Re = G00 + s_re G11, Im = s_01 G01 + s_10 G10
 };
 
-__device__ __forceinline__ void ab_epilogue(uint64_t* tmem_bar, uint32_t tmem_base, float2* staging,
-                                            AbTcParams const& P, int batch, int I, int J0, int nb,
-                                            int warp, int lane) {
-	mbar_wait(tmem_bar, 0);
-	asm volatile("tcgen05.fence::after_thread_sync;");
-	const int quarter = warp & 3;
-	const int m = quarter * 32 + lane;
-	const int il = m >> 1, par = m & 1;
-	float* stf = (float*)staging;
-	const int te = threadIdx.x - 64;
+__global__ void __launch_bounds__(TC_THREADS, 1)
+ab_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, AbTcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	const int batch = blockIdx.y;
+	const int I = blockIdx.x / P.njj, J0 = 2 * (blockIdx.x % P.njj);
+	const int nb = ((J0 + 1) * 64 < P.N) ? 2 : 1;
+	const int nk = (P.K + TC_KT - 1) / TC_KT;
+	int acc[2][64];
+	if( !tc_mainloop(tc_smem, &tmap_a, &tmap_b, 128 * I, P.a_batched ? batch : 0, 128 * J0, batch, nb, 0, nk, acc) )
+		return;
+
+	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
+	float2* staging = (float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
 	float2* cb = P.c + (long)batch * P.c_batch;
-	for( int h=0; h<nb; ++h ) {
-		const int J = J0 + h;
-#pragma unroll 1
-		for( int c0=0; c0<128; c0+=32 ) {
-			uint32_t r[32];
-			const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(128 * h + c0);
-			asm volatile(
-				"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-				"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-				"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-				: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-				  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-				  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-				  "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-				: "r"(taddr));
-			asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+	const float s_re = P.s_re, s_01 = P.s_01, s_10 = P.s_10;
 #pragma unroll
-			for( int q=0; q<16; ++q ) {
-				// even row 2m: (G00, G01); odd row 2m+1: (G10, G11); swap the second entries
-				const int mine0 = (int)r[2*q], mine1 = (int)r[2*q+1];
-				const int other1 = __shfl_xor_sync(0xffffffffu, mine1, 1);
-				const float v = par ? (P.s_01 * (float)other1 + P.s_10 * (float)mine0)
-				                    : ((float)mine0 + P.s_re * (float)other1);
-				const int jl = (c0 >> 1) + q;
-				stf[(il * 65 + jl) * 2 + par] = v;
-			}
-		}
-		asm volatile("bar.sync 1, 128;" ::: "memory");
-		for( int idx = te; idx < 64 * 64; idx += 128 ) {
+	for( int h=0; h<2; ++h ) {
+		if( h >= nb ) break;
+		const int J = J0 + h;
+		// even row 2m: (G00, G01); odd row 2m+1: (G10, G11); the partner's second entry
+		tc_stage(acc[h], staging, [=](int mine0, int other1, int par) {
+			return par ? (s_01 * (float)other1 + s_10 * (float)mine0) : ((float)mine0 + s_re * (float)other1); });
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
+		for( int idx = threadIdx.x; idx < 64 * 64; idx += TC_CONSUMERS ) {
 			const int il2 = idx >> 6, jl2 = idx & 63;
 			const int i = I * 64 + il2, j = J * 64 + jl2;
 			if( i < P.M && j < P.N ) {
@@ -551,93 +443,7 @@ __device__ __forceinline__ void ab_epilogue(uint64_t* tmem_bar, uint32_t tmem_ba
 				*dst = o;
 			}
 		}
-		asm volatile("bar.sync 1, 128;" ::: "memory");
-	}
-}
-
-template<int TC_STAGES>
-__global__ void __launch_bounds__(TC_THREADS)
-ab_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, AbTcParams P) {
-	extern __shared__ __align__(1024) unsigned char tc_smem[];
-	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
-	float2* staging = (float2*)(tiles + TC_STAGES * TC_STAGE_BYTES);
-	uint64_t* full_bar  = (uint64_t*)(staging + 64 * 65);
-	uint64_t* empty_bar = full_bar + TC_STAGES;
-	uint64_t* tmem_bar  = empty_bar + TC_STAGES;
-	uint32_t* tmem_slot = (uint32_t*)(tmem_bar + 1);
-
-	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const int batch = blockIdx.y;
-	const int I = blockIdx.x / P.njj, J0 = 2 * (blockIdx.x % P.njj);
-	const int nb = ((J0 + 1) * 64 < P.N) ? 2 : 1;
-	const int nk = (P.K + TC_KT - 1) / TC_KT;
-
-	if( threadIdx.x == 0 ) {
-		for( int s=0; s<TC_STAGES; ++s ) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-		mbar_init(tmem_bar, 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	if( warp == 1 ) {
-		asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-		             :: "r"(smem_u32(tmem_slot)), "n"(256));
-		asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	asm volatile("tcgen05.fence::after_thread_sync;");
-	const uint32_t tmem_base = *tmem_slot;
-
-	if( warp == 0 ) {
-		if( lane == 0 ) {
-			const uint32_t bytes = (uint32_t)TC_TILE_BYTES * (1 + nb);
-			for( int it=0; it<nk; ++it ) {
-				const int s = it % TC_STAGES;
-				const uint32_t ph = (it / TC_STAGES) & 1;
-				mbar_wait(&empty_bar[s], ph ^ 1);
-				unsigned char* a = tiles + (size_t)s * TC_STAGE_BYTES;
-				mbar_expect_tx(&full_bar[s], bytes);
-				tma_load_3d(a, &tmap_a, &full_bar[s], 128 * I, it * TC_KT, P.a_batched ? batch : 0);
-				tma_load_3d(a + TC_TILE_BYTES, &tmap_b, &full_bar[s], 128 * J0, it * TC_KT, batch);
-				if( nb == 2 ) tma_load_3d(a + 2 * TC_TILE_BYTES, &tmap_b, &full_bar[s], 128 * (J0 + 1), it * TC_KT, batch);
-			}
-		}
-	} else if( warp == 1 ) {
-		const uint32_t idesc = umma_idesc_i8(nb == 2 ? 256u : 128u);
-		for( int it=0; it<nk; ++it ) {
-			const int s = it % TC_STAGES;
-			const uint32_t ph = (it / TC_STAGES) & 1;
-			mbar_wait(&full_bar[s], ph);
-			asm volatile("tcgen05.fence::after_thread_sync;");
-			if( lane == 0 ) {
-				const uint32_t a_addr = smem_u32(tiles + (size_t)s * TC_STAGE_BYTES);
-				const uint32_t b_addr = a_addr + TC_TILE_BYTES;
-#pragma unroll
-				for( int kk=0; kk<TC_KT/32; ++kk ) {
-					const uint64_t da = umma_desc_mn_sw128(a_addr + kk * 32 * 128);
-					const uint64_t db = umma_desc_mn_sw128(b_addr + kk * 32 * 128);
-					const uint32_t acc = (it > 0 || kk > 0) ? 1u : 0u;
-					asm volatile(
-						"{\n\t.reg .pred p;\n\t"
-						"setp.ne.b32 p, %4, 0;\n\t"
-						"tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-						:: "r"(tmem_base), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-				}
-				asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-				             :: "r"(smem_u32(&empty_bar[s])) : "memory");
-				if( it == nk - 1 ) {
-					asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-					             :: "r"(smem_u32(tmem_bar)) : "memory");
-				}
-			}
-			__syncwarp();
-		}
-	} else {
-		ab_epilogue(tmem_bar, tmem_base, staging, P, batch, I, J0, nb, warp, lane);
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;");
-	__syncthreads();
-	if( warp == 1 ) {
-		asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(256));
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
 	}
 }
 
@@ -732,7 +538,7 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 			cuuint32_t box[3] = {128, TC_KT, 1};
 			cuuint32_t estr[3] = {1, 1, 1};
 			CUresult res = get_encode_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ub, gdim, gstr,
-			                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+			                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
 			                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 			if( res != CUDA_SUCCESS ) use_tc = false;
 			if( use_tc ) {
@@ -743,34 +549,11 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 				P.ntile = 0;
 				for( int i=0; i<T; ++i ) P.ntile += i / 2 + 1;     // (row block, column-block pair) units
 				P.alpha = (float)alpha; P.beta = (float)beta; P.conj_u = conj_u;
-				static const bool use_cluster = getenv("BFB_LINALG_CLUSTER") != nullptr;
-				static const int  nstage = getenv("BFB_LINALG_STAGES") ? atoi(getenv("BFB_LINALG_STAGES")) : 3;
-				auto smem_for = [](int stages) {
-					return (size_t)stages * TC_STAGE_BYTES + 64 * 65 * sizeof(float2) +
-					       (2 * stages + 1) * sizeof(uint64_t) + 16 + 1024;   // + 1024: alignment of the window
-				};
-				if( use_cluster && T >= 2 ) {
-					int TT = (T + 1) / 2;                           // 256-row super blocks
-					size_t smem = smem_for(TC2_STAGES);
-					BFB_CUDA(cudaFuncSetAttribute(corr_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-					                              (int)smem), BF_STATUS_INTERNAL_ERROR);
-					dim3 grid2(2 * (TT * (TT + 1) / 2), (unsigned)kb);
-					corr_tc2_kernel<<<grid2, TC_THREADS, smem, st>>>(tmap, P);
-				} else {
-					dim3 grid(P.ntile, (unsigned)kb);
-#define BFB_TC_LAUNCH(S_) do { size_t smem = smem_for(S_); \
-						BFB_CUDA(cudaFuncSetAttribute(corr_tc_kernel<S_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-						                              (int)smem), BF_STATUS_INTERNAL_ERROR); \
-						corr_tc_kernel<S_><<<grid, TC_THREADS, smem, st>>>(tmap, P); } while(0)
-					switch( nstage ) {
-					case 2:  BFB_TC_LAUNCH(2); break;
-					case 4:  BFB_TC_LAUNCH(4); break;
-					case 5:  BFB_TC_LAUNCH(5); break;
-					case 8:  BFB_TC_LAUNCH(8); break;
-					default: BFB_TC_LAUNCH(3); break;
-					}
-#undef BFB_TC_LAUNCH
-				}
+				const size_t smem = tc_smem_bytes();
+				BFB_CUDA(cudaFuncSetAttribute(corr_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+				                              (int)smem), BF_STATUS_INTERNAL_ERROR);
+				dim3 grid(P.ntile, (unsigned)kb);
+				corr_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tmap, P);
 				count_launch();
 				BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 				continue;
@@ -913,14 +696,14 @@ static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFsta
 		cuuint64_t gdim[3] = {(cuuint64_t)(2 * P.M), (cuuint64_t)P.K, (cuuint64_t)na};
 		cuuint64_t gstr[2] = {(cuuint64_t)pitch, (cuuint64_t)((long)P.K * pitch)};
 		if( get_encode_fn()(&ta, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, h->at_buf, gdim, gstr, box, estr,
-		                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+		                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
 		                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS ) return false;
 	}
 	{
 		cuuint64_t gdim[3] = {(cuuint64_t)(2 * P.N), (cuuint64_t)P.K, (cuuint64_t)nbatch};
 		cuuint64_t gstr[2] = {(cuuint64_t)P.b.sk, (cuuint64_t)(P.nb == 1 ? P.b.sb[0] : round_up<long>(P.b.sk * P.K, 16))};
 		if( get_encode_fn()(&tb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)P.b.p, gdim, gstr, box, estr,
-		                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+		                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
 		                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS ) return false;
 	}
 	AbTcParams Q;
@@ -933,13 +716,12 @@ static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFsta
 	Q.s_re = (ca != cb) ? 1.f : -1.f;
 	Q.s_01 = cb ? -1.f : 1.f;
 	Q.s_10 = ca ? -1.f : 1.f;
-	constexpr int STAGES = 3;
-	const size_t smem = (size_t)STAGES * TC_STAGE_BYTES + 64 * 65 * sizeof(float2) + (2 * STAGES + 1) * sizeof(uint64_t) + 16 + 1024;
-	if( cudaFuncSetAttribute(ab_tc_kernel<STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
+	const size_t smem = tc_smem_bytes();
+	if( cudaFuncSetAttribute(ab_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
 		*status = BF_STATUS_INTERNAL_ERROR; return true;
 	}
 	dim3 grid((unsigned)(div_up<int>(P.M, 64) * Q.njj), (unsigned)nbatch);
-	ab_tc_kernel<STAGES><<<grid, TC_THREADS, smem, st>>>(ta, tb, Q);
+	ab_tc_kernel<<<grid, TC_THREADS, smem, st>>>(ta, tb, Q);
 	count_launch();
 	if( cudaGetLastError() != cudaSuccess ) *status = BF_STATUS_INTERNAL_ERROR;
 	return true;

@@ -1,4 +1,4 @@
-// map.cu -- fixed sm_100a kernels for the element-wise expressions that the
+// map.cu -- fixed sm_90a kernels for the element-wise expressions that the
 // hot-path blocks hand to bfMap, plus a bfMap front end that recognises them.
 //
 // Replaces (for these expressions only): src/map.cpp:630-797 (bfMap, NVRTC
@@ -450,7 +450,7 @@ BFstatus bfMap(int ndim, long const* shape, char const* const* axis_names,
 	);
 }
 
-// B200 extension (test hook): compiles the kernel bfMap would run for this
+// Extension (test hook): compiles the kernel bfMap would run for this
 // call and stops; works without a device.  *mode = 0: array names are plain
 // element references, 1: callable views.
 BFstatus bfMapCompile(int ndim, long const* shape, char const* const* axis_names,

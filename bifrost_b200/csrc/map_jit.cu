@@ -1,5 +1,5 @@
 // map_jit.cu -- the general bfMap: an arbitrary user expression over named
-// arrays, compiled at run time with NVRTC for sm_100a and cached.
+// arrays, compiled at run time with NVRTC for sm_90a and cached.
 //
 // Replaces src/map.cpp:110-406,630-797 (code generation, NVRTC build, kernel
 // cache, launch) and the device headers it embeds (src/Complex.hpp,
@@ -356,7 +356,7 @@ static BFstatus nvrtc_compile(std::string const& src, std::string const& name, s
 	if( !jit_load_nvrtc() ) { if( log ) *log = g_jit.why; return BF_STATUS_UNSUPPORTED; }
 	nvrtcProgram_t prog = nullptr;
 	if( g_jit.nvrtcCreateProgram(&prog, src.c_str(), name.c_str(), 0, nullptr, nullptr) != 0 ) return BF_STATUS_INTERNAL_ERROR;
-	const char* opts[] = { "--std=c++17", "--gpu-architecture=sm_100a", "--use_fast_math",
+	const char* opts[] = { "--std=c++17", "--gpu-architecture=sm_90a", "--use_fast_math",
 	                       "--device-as-default-execution-space", "--restrict", "-w" };
 	int rc = g_jit.nvrtcCompileProgram(prog, (int)(sizeof(opts) / sizeof(opts[0])), opts);
 	if( log ) {

@@ -1,4 +1,4 @@
-// reduce.cu -- bfReduce for sm_100a.
+// reduce.cu -- bfReduce for sm_90a.
 //
 // Replaces: src/reduce.cu:881-920 (entry), :251-345 (real dispatch),
 // :62-121,156-212 (real kernels), :366-484 (complex standard),

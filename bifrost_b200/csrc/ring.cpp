@@ -23,7 +23,7 @@
 // condition variable per ring order everything; all blocking calls are
 // predicates on (head, tail, reserve head, guarantees, open spans).
 //
-// Placement (the B200 host has two sockets, each with four GPUs behind it):
+// Placement (multi-socket hosts with GPUs behind each socket):
 // bfRingSetAffinity(core) makes later allocations of a host-space ring come
 // from the NUMA node of that core -- for pinned rings that is the node whose
 // PCIe root the consuming GPU hangs off (the reference needs hwloc for this

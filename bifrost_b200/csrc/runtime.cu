@@ -110,7 +110,7 @@ const char* bfGetSpaceString(BFspace space) {
 	}
 }
 
-// B200 extension: CUDA IPC for device allocations of bfMalloc (space 'cuda'), so
+// Extension: CUDA IPC for device allocations of bfMalloc (space 'cuda'), so
 // that cooperating processes -- one per GPU -- can map each other's buffers
 // (peer access over NVLink is enabled when the handle is opened).  The handle is
 // the 64-byte cudaIpcMemHandle_t; `ptr` must be the start of the allocation.

@@ -1,5 +1,5 @@
 // spectrometer.cu -- bfSpectrometerFused: the GUPPI spectrometer gulp as ONE
-// kernel (B200 extension; no single reference counterpart).
+// kernel (extension; no single reference counterpart).
 //
 // Equivalent reference chain (testbench/gpuspec_simple.py:44-55, README):
 //   transpose([time,pol,freq,fine_time])           bfTranspose

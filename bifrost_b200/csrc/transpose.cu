@@ -1,4 +1,4 @@
-// transpose.cu -- bfTranspose for sm_100a.
+// transpose.cu -- bfTranspose for sm_90a.
 //
 // Replaces: src/transpose.cu:503-561 (dispatch), :65-247 +
 // src/transpose_gpu_kernel.cuh:65-147 (32x32 tile kernel) and the three

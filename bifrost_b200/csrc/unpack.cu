@@ -1,4 +1,4 @@
-// unpack.cu -- bfUnpack for sm_100a (device arrays; system-space arrays are
+// unpack.cu -- bfUnpack for sm_90a (device arrays; system-space arrays are
 // unpacked by a host loop with the reference's CPU convention, as its ABI does).
 //
 // Replaces: src/unpack.cpp:242-535 (entry + dtype dispatch) with the device

@@ -1,5 +1,5 @@
 """bf.fdmt.Fdmt (mirrors python/bifrost/fdmt.py:38-76 -> bfFdmt*), plus the
-sharded full-band form (B200 extension, bfFdmtShard*)."""
+sharded full-band form (extension, bfFdmtShard*)."""
 import ctypes
 
 import numpy as np
@@ -37,7 +37,7 @@ class Fdmt(BifrostObject):
                                  workspace_ptr, size))
         return odata
 
-    # ---- sharded full-band transform (B200 extension; include/bifrost_b200.h) ----
+    # ---- sharded full-band transform (extension; include/bifrost_b200.h) ----
     def shard_init(self, rank, nrank):
         """This plan (initialised with the FULL band) becomes rank `rank` of
         `nrank` cooperating plans."""

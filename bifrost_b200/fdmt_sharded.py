@@ -1,4 +1,4 @@
-"""Full-band FDMT across GPUs (B200 extension; SURVEY 8f.1, DESIGN 6).
+"""Full-band FDMT across GPUs (extension; SURVEY 8f.1, DESIGN 6).
 
 The reference scales FDMT by giving every GPU an independent frequency
 sub-band (python/bifrost/blocks/fdmt.py:59-124 on a `gpu=` block each); the

@@ -2,7 +2,7 @@
 behind the hot-path expressions.
 
 ``bf.map`` takes an arbitrary C++ expression over named arrays, like the
-reference's: the library compiles it at run time with NVRTC for sm_100a
+reference's: the library compiles it at run time with NVRTC for sm_90a
 (csrc/map_jit.cu).  The two expression families the hot-path blocks use -- the
 detect products (blocks/detect.py:87-136) and the accumulate update
 (blocks/accumulate.py:67) -- are recognised and run as compiled kernels

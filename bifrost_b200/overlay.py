@@ -1,4 +1,4 @@
-"""Overlay of the B200 hot path on a stock libbifrost binding.
+"""Overlay of the H100 hot path on a stock libbifrost binding.
 
 The reference's Python package binds ``libbifrost.so`` through a ctypes
 namespace (``bifrost/libbifrost.py:38-40``: ``import

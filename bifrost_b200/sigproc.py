@@ -52,8 +52,13 @@ def machine2id(name):
 
 
 def _write_string(f, text):
-    f.write(struct.pack('=i', len(text)))
-    f.write(text.encode())
+    raw = text.encode()
+    # sigproc readers (_read_string here, sigproc2.py:175 of the reference) stop
+    # at a string of 80 bytes or more: such a header could not be read back
+    if len(raw) >= 80:
+        raise ValueError("sigproc header string of %d bytes (at most 79): %r" % (len(raw), text))
+    f.write(struct.pack('=i', len(raw)))
+    f.write(raw)
 
 
 def write_header(hdr, f):

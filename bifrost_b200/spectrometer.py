@@ -1,4 +1,4 @@
-"""bf.spectrometer: the fused GUPPI spectrometer gulp (B200 extension).
+"""bf.spectrometer: the fused GUPPI spectrometer gulp (extension).
 
 One kernel for transpose -> fft(fine_time, fftshift) -> detect('stokes') ->
 reduce(freq, f_avg) -> accumulate(nframe) (testbench/gpuspec_simple.py:44-55).

@@ -1,4 +1,4 @@
-/* bifrost_b200.h -- C ABI of the B200-native Bifrost hot path.
+/* bifrost_b200.h -- C ABI of the H100-native (sm_90a) Bifrost hot path.
  *
  * One consolidated header for the drop-in boundary.  Every type, enum value
  * and entry point below is what the reference's ctypes FFI binds for the
@@ -241,7 +241,7 @@ BFstatus bfFftDestroy(BFfft plan);
 /* ------------------------------------------------------------------ *
  * LinAlg                              (ref: src/bifrost/linalg.h:43-54)
  * c = alpha*a.b + beta*c;  b==NULL: a.a^H;  a==NULL: b^H.b.
- * The a.a^H / b^H.b forms write the lower triangle only (tcgen05 int8 path for
+ * The a.a^H / b^H.b forms write the lower triangle only (wgmma int8 path for
  * ci8).  a.b is a general strided SIMT product (ci8/ci16/cf32/f32 with float
  * accumulation, f64/cf64 with double; conjugated views honoured).
  * ------------------------------------------------------------------ */
@@ -269,7 +269,7 @@ BFstatus bfQuantize(BFarray const* in, BFarray const* out, double scale);
 /* ------------------------------------------------------------------ *
  * Map                                  (ref: src/bifrost/map.h:82-94)
  * The reference JIT-compiles `func` with NVRTC.  This build ships fixed
- * sm_100a kernels for the expressions the hot-path blocks emit (detect:
+ * sm_90a kernels for the expressions the hot-path blocks emit (detect:
  * python/bifrost/blocks/detect.py:87-136; accumulate:
  * python/bifrost/blocks/accumulate.py:67) and returns
  * BF_STATUS_UNSUPPORTED for any other expression.
@@ -351,7 +351,7 @@ BFstatus bfFdmtPackedMegaQuery(BFsize nchan, BFsize max_delay, double f0, double
                               double exponent, long ntime, long* header, int* tmpl);
 
 /* B200 extension (test hook): compiles the kernel bfMap would run for this
- * call (NVRTC, sm_100a) and stops; needs no device.  *mode = 0: the array
+ * call (NVRTC, sm_90a) and stops; needs no device.  *mode = 0: the array
  * names are plain element references, 1: callable views (src/map.cpp:712-735
  * tries them in this order). */
 BFstatus bfMapCompile(int ndim, long const* shape, char const* const* axis_names,

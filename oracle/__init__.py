@@ -12,7 +12,7 @@ Pinning status (see DESIGN.md "Oracle"):
   transpose   numpy.transpose IS the reference's CPU path (blocks/transpose.py:80)
   reduce      numpy definition of test/test_reduce.py:47-65
   fft         numpy.fft in fp64 is the reference's own gold (test/test_fft.py:42-51)
-  fdmt        pinned against the reference CUDA library built for sm_100 and run
+  fdmt        pinned against the reference CUDA library built for sm_90a and run
               under gpurun (oracle/ref_build.sh -> oracle/_ref/); golden outputs
               committed under tests/golden/ by tests/golden/make_fdmt_golden.py
   quantize    pinned by the known answers of test/test_quantize.py:33-50

@@ -1,6 +1,7 @@
 #!/bin/bash
 # Builds the UNMODIFIED reference CUDA sources of the hot path, where they lie
-# under /root/reference/src, into oracle/_ref/libbifrost_ref.so for sm_100.
+# under $REF/src (a checkout of the reference), into oracle/_ref/libbifrost_ref.so
+# for sm_90a.
 # TEST INFRASTRUCTURE: used by tests/ (GPU parity against the real reference)
 # and as the "kernel to beat" in benchmarks/compare_ref.py.  Nothing under
 # bifrost_b200/ links or loads it.
@@ -60,7 +61,7 @@ extern "C" BFstatus bfMap(int, long const*, char const*const*, int, BFarray cons
 extern "C" BFstatus bfMapClearCache() { return BF_STATUS_SUCCESS; }
 EOF
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100,code=sm_100 -O3 -std=c++17 -Xcompiler -fPIC -w \
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Xcompiler -fPIC -w \
        -I$OUT/include -I$REF/src -DBF_CUDA_ENABLED=1"
 SRCS="common.cpp memory.cpp array.cpp cuda.cpp fdmt.cu reduce.cu transpose.cu \
       linalg.cu linalg_kernels.cu unpack.cpp gunpack.cu quantize.cpp guantize.cu"
@@ -74,6 +75,6 @@ for s in $SRCS; do
 done
 $NVCC $FLAGS -c $OUT/obj/map_stub.cpp -o $OUT/obj/map_stub.o
 for p in $pids; do wait $p; done
-$NVCC -gencode arch=compute_100,code=sm_100 -shared -o $OUT/libbifrost_ref.so \
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o $OUT/libbifrost_ref.so \
       $OBJS $OUT/obj/map_stub.o -lcublas
 echo "ref_build: wrote $OUT/libbifrost_ref.so"

@@ -2,9 +2,8 @@
 
 `-m "not gpu"` tests run on a CPU-only box: oracle vs golden vectors, host
 logic, C-ABI exports.  `-m gpu` tests are the parity tests proper: they drive
-libbifrost_b200.so through the Python/ctypes boundary on a real B200 and
-compare with the oracle (and, when oracle/_ref/libbifrost_ref.so travelled
-with the snapshot, with the reference's own CUDA code).
+libbifrost_b200.so through the Python/ctypes boundary on a real H100 and
+compare with the oracle (and with stored outputs of the reference's own CUDA code).
 """
 import os
 import subprocess
@@ -23,7 +22,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a machine with an H100)")
     lib = os.path.join(ROOT, 'bifrost_b200', 'lib', 'libbifrost_b200.so')
     if not os.path.exists(lib):
         # Building the product library is allowed from tests (it is never *used*

@@ -1,12 +1,14 @@
 """Generates tests/golden/fdmt_ref_golden.npz by running the REFERENCE's own
-CUDA FDMT (oracle/_ref/libbifrost_ref.so, built from /root/reference/src by
-oracle/ref_build.sh) on seeded inputs.  Needs a GPU:
+CUDA FDMT (oracle/_ref/libbifrost_ref.so, built by oracle/ref_build.sh) on
+seeded inputs.  Needs a GPU:
 
-    gpurun -- 'python tests/golden/make_fdmt_golden.py gpurun_out/fdmt_ref_golden.npz'
+    bash oracle/ref_build.sh && python tests/golden/make_fdmt_golden.py OUT.npz
 
-then copy the file to tests/golden/.  The reference's tests hold no FDMT
+then copy OUT.npz to tests/golden/.  The reference's tests hold no FDMT
 known-answer vector (test/test_fdmt.py:49-65 is a smoke test), so these
-outputs are what pins the oracle (oracle/fdmt.py) for this op.
+outputs are what pins the oracle (oracle/fdmt.py) for this op.  The inputs are
+regenerated from their seeds (`make_input`); of each output a fixed seeded
+sample of elements is stored (`golden_index`), which keeps the file small.
 """
 import ctypes
 import os
@@ -32,6 +34,12 @@ CASES = [
     ('t640_c256_d100_i16', 640, 256, 100, 1200., 300. / 256, 'i16', ()),
 ]
 SENTINEL = -999.0
+
+
+def golden_index(i, size):
+    """Flat indices of case i's output kept in the golden file."""
+    from golden.make_ref_gpu_golden import sample_index
+    return sample_index(size, 4000 + i)
 
 
 def make_input(name, shape, dtype, seed):
@@ -67,12 +75,12 @@ def main(out_path):
         bf.device.stream_synchronize()
         out = d_out.copy('system')
         _check(ref.bfFdmtDestroy(plan))
-        store[name + '/in'] = x
-        store[name + '/out'] = np.asarray(out)
+        out = np.asarray(out).ravel()
+        store[name + '/out'] = out[golden_index(i, out.size)]
         print(name, 'ok', np.asarray(out).shape)
     np.savez_compressed(out_path, **store)
     print('wrote', out_path)
 
 
 if __name__ == '__main__':
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, 'gpurun_out', 'fdmt_ref_golden.npz'))
+    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, 'tests', 'golden', 'fdmt_ref_golden.npz'))

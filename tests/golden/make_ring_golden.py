@@ -22,20 +22,23 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 import ringtrace  # noqa: E402
 
 SEEDS = [(11, 260), (12, 260), (13, 260), (14, 260), (15, 260), (16, 260)]
+# the longer scripts of tests/test_ring.py::test_live_differential_against_the_reference_ring
+LIVE_SEEDS = [(seed, 350) for seed in range(100, 112)]
 
 
 def main():
     ref = ringtrace.load_reference()
     assert ref is not None, 'build oracle/_ref/libbifrost_ref_ring.so first (oracle/ref_ring_build.sh)'
-    cases = []
-    for seed, nstep in SEEDS:
-        script, trace = ringtrace.generate(ref, seed, nstep)
-        cases.append(dict(seed=seed, script=script, trace=trace))
-        print(seed, len(script), 'calls')
+    cases, live = [], []
+    for seeds, into in ((SEEDS, cases), (LIVE_SEEDS, live)):
+        for seed, nstep in seeds:
+            script, trace = ringtrace.generate(ref, seed, nstep)
+            into.append(dict(seed=seed, script=script, trace=trace))
+            print(seed, len(script), 'calls')
     out = os.path.join(HERE, 'ring_traces.json.gz')
     with gzip.GzipFile(out, 'wb', mtime=0) as f:
         f.write(json.dumps(dict(source='reference src/ring_impl.cpp via oracle/ref_ring_build.sh',
-                                cases=cases), separators=(',', ':')).encode())
+                                cases=cases, live=live), separators=(',', ':')).encode())
     print('wrote', out, os.path.getsize(out), 'bytes')
 
 

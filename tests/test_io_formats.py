@@ -124,6 +124,26 @@ def test_sigproc_filterbank_round_trip(tmp_path, dtype, npdt):
     np.testing.assert_array_equal(np.concatenate(out.chunks, 0), x)
 
 
+def test_sigproc_sink_keeps_the_file_name_of_a_long_source_path(tmp_path):
+    """The GUPPI reader hands the whole path it read on as `rawdatafile`; a path
+    of 80 bytes or more is not a string a sigproc header can hold, so the sink
+    writes the file name and the header reads back."""
+    x = np.arange(20 * 2 * 8, dtype=np.float32).reshape(20, 2, 8)
+    hdr = fil_header(8, 2, 'f32')
+    hdr['rawdatafile'] = '/' + 'd' * 120 + '/volt.raw'
+    with Pipeline() as p:
+        src = blocks.array_source(x, hdr, gulp_nframe=16)
+        blocks.write_sigproc(src, path=str(tmp_path))
+        p.run()
+    with open(str(tmp_path / 'obs.fil'), 'rb') as f:
+        h = sigproc.read_header(f)
+        body = np.fromfile(f, dtype=np.float32)
+    assert h['rawdatafile'] == 'volt.raw'
+    np.testing.assert_array_equal(body.reshape(x.shape), x)
+    with pytest.raises(ValueError):
+        sigproc.write_header(dict(source_name='x' * 80), io.BytesIO())
+
+
 def test_sigproc_file_without_id_cards_round_trips(tmp_path):
     """read_sigproc -> write_sigproc of a file that has no telescope_id / machine_id
     card: the ids come back as 'unknown' and the sink leaves the cards out again

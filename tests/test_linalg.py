@@ -229,7 +229,7 @@ def test_matmul_ab_ci8_and_beamformer():
 @pytest.mark.parametrize("m,n,k,batch", [(5, 64, 32, None), (64, 128, 64, None), (111, 224, 77, None),
                                          (65, 136, 500, 3), (200, 1000, 300, 2), (32, 4096, 512, 4)])
 def test_matmul_ab_ci8_on_the_tensor_cores(m, n, k, batch):
-    """ci8 x ci8 -> cf32 with TMA-friendly operands takes the tcgen05 kernel
+    """ci8 x ci8 -> cf32 with TMA-friendly operands takes the wgmma kernel
     (two launches: a^T staging + the product); exact integers, every
     conjugation flag, alpha / beta, a shared or per-batch weight matrix."""
     rng = np.random.default_rng(m * n + k)
@@ -316,29 +316,18 @@ def test_baseline_config4_full_size_against_the_oracle(ntime):
 
 @pytest.mark.gpu
 def test_correlator_matches_the_reference_library():
-    """Same BFarray structs through the reference's own bfLinAlgMatMul
-    (oracle/_ref, src/linalg.cu:242-357 + linalg_kernels.cu) and ours."""
-    import ctypes
-    import reflib
-    ref = reflib.load()
-    if ref is None or not hasattr(ref, 'bfLinAlgMatMul'):
-        pytest.skip("oracle/_ref/libbifrost_ref.so not present")
-    from bifrost_b200.libbifrost import _check
-    rng = np.random.default_rng(77)
-    for (ntime, nchan, n) in [(64, 3, 32), (512, 4, 512), (200, 2, 130)]:
-        x = rand_ci8(rng, (ntime, nchan, n))
-        ours = run_bhb(x)
-        d_x = bf.asarray(x, space='cuda')
-        xv = d_x.transpose((1, 0, 2))
-        d_c = bf.zeros((nchan, n, n), 'cf32', 'cuda')
-        h = ctypes.c_void_p()
-        _check(ref.bfLinAlgCreate(ctypes.byref(h)))
-        _check(ref.bfLinAlgMatMul(h, 1.0, None, xv.as_BFarray(), 0.0, d_c.as_BFarray()))
-        _check(ref.bfStreamSynchronize())
-        theirs = np.asarray(d_c.copy('system'))
-        _check(ref.bfLinAlgDestroy(h))
-        il = np.tril_indices(n)
-        a, b = ours[:, il[0], il[1]], theirs[:, il[0], il[1]]
+    """The same inputs through the reference's own bfLinAlgMatMul
+    (src/linalg.cu:242-357 + linalg_kernels.cu) gave the stored outputs
+    (tests/golden/make_ref_gpu_golden.py); ours against them."""
+    import sys
+    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+    from golden import make_ref_gpu_golden as refgold
+    gold = refgold.load()
+    for ci, x in enumerate(refgold.linalg_inputs()):
+        ntime = x.shape[0]
+        ours = refgold.linalg_lower(run_bhb(x)).ravel()
+        a = ours[refgold.sample_index(ours.size, 2000 + ci)]
+        b = gold['linalg/%d' % ci]
         # The reference accumulates (x/127)(y/127) in fp32 and rounds x127^2 at the end
         # (linalg_kernels.cu:94-112): exact only while the rounding errors stay below
         # one half -- short integrations.  Ours is integer-exact (checked against the

@@ -1,7 +1,7 @@
 """General bfMap (csrc/map_jit.cu): the reference's own test expressions
 (test/test_map.py) and the examples of python/bifrost/map.py:96-112.
 
-CPU: every expression must COMPILE for sm_100a (bfMapCompile needs no device)
+CPU: every expression must COMPILE for sm_90a (bfMapCompile needs no device)
 in the form the reference would pick -- plain element references first,
 callable views when the string indexes its arrays.  GPU: the numerics of the
 reference's tests, value for value.

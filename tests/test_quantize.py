@@ -79,7 +79,7 @@ def _packed_case(nbit, cplx, n=4096 * 8 + 24):
 def test_gpu_packed_outputs_match_oracle_and_reference(odtype, nbit, scale):
     import sys, os
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    import reflib
+    from golden import make_ref_gpu_golden as refgold
     cplx = odtype.startswith('c')
     x = _packed_case(nbit, cplx)
     d_in = bf.asarray(x, space='cuda')
@@ -90,19 +90,16 @@ def test_gpu_packed_outputs_match_oracle_and_reference(odtype, nbit, scale):
     got = np.asarray(d_raw.copy('system'))
     want = oquant.quantize_packed(x, nbit, scale)
     np.testing.assert_array_equal(got, want)
-    # the reference's own GPU kernels, when oracle/_ref travelled (1-bit: on the
-    # bits its masks keep -- see oracle/quantize.py)
-    ref = reflib.load()
-    if ref is not None and hasattr(ref, 'bfQuantize'):
-        d_raw2 = bf.asarray(np.zeros(nbyte, np.uint8), space='cuda')
-        d_out2 = bf.ndarray(space='cuda', buffer=d_raw2.ctypes.data, shape=x.shape, dtype=odtype)
-        # (the reference's contiguity test rejects the byte strides of real
-        # sub-byte arrays -- BF_STATUS_UNSUPPORTED_STRIDE; the complex ones go through)
-        if ref.bfQuantize(d_in.as_BFarray(), d_out2.as_BFarray(), float(scale)) == 0:
-            bf.device.stream_synchronize()
-            theirs = np.asarray(d_raw2.copy('system'))
-            mask = oquant.reference_1bit_mask if nbit == 1 else 0xFF
-            np.testing.assert_array_equal(got & mask, theirs & mask)
+    # what the reference's own GPU kernels wrote for this input (1-bit: on the
+    # bits its masks keep -- see oracle/quantize.py).  The reference's contiguity
+    # test rejects the byte strides of most sub-byte arrays (it answers
+    # BF_STATUS_UNSUPPORTED_STRIDE), so only ci4 has stored outputs.
+    gold = refgold.load()
+    key = refgold.quantize_key(odtype, scale)
+    assert (key in gold.files) == (odtype == 'ci4')
+    if key in gold.files:
+        mask = oquant.reference_1bit_mask if nbit == 1 else 0xFF
+        np.testing.assert_array_equal(got & mask, gold[key] & mask)
 
 
 @pytest.mark.gpu

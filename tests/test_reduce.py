@@ -126,32 +126,24 @@ def test_errors():
 
 
 def test_reduce_matches_the_reference_library():
-    """Same BFarray structs through the reference's own bfReduce (oracle/_ref,
-    src/reduce.cu:881-920) and ours: bit-identical for sum / min / max on float
-    data (same left-to-right order), 1 ulp for mean / stderr."""
+    """The same inputs through the reference's own bfReduce (src/reduce.cu:881-920)
+    gave the stored outputs (tests/golden/make_ref_gpu_golden.py): ours are
+    bit-identical for sum / min / max on float data (same left-to-right order),
+    within 1 ulp for mean."""
     import os
     import sys
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    import reflib
-    ref = reflib.load()
-    if ref is None or not hasattr(ref, 'bfReduce'):
-        pytest.skip("oracle/_ref/libbifrost_ref.so not present")
-    from bifrost_b200.libbifrost import _bf, _check
-    rng = np.random.default_rng(11)
-    ops = dict(sum=_bf.BF_REDUCE_SUM, min=_bf.BF_REDUCE_MIN, max=_bf.BF_REDUCE_MAX, mean=_bf.BF_REDUCE_MEAN,
-               pwrsum=_bf.BF_REDUCE_POWER_SUM)
-    for shape, axis, n in [((4096, 256), 1, 4), ((4096, 256), 0, 8), ((4, 65536), 1, 4), ((20, 40, 60), 1, 5)]:
-        a = rng.normal(size=shape).astype(np.float32)
-        oshape = list(shape)
-        oshape[axis] //= n
+    from golden import make_ref_gpu_golden as refgold
+    gold = refgold.load()
+    for ci, a in enumerate(refgold.reduce_inputs()):
+        shape, axis, n = refgold.REDUCE_CASES[ci]
         d_a = bf.asarray(a, space='cuda')
-        for name, code in ops.items():
-            d_o = bf.empty(oshape, 'f32', 'cuda')
-            d_r = bf.empty(oshape, 'f32', 'cuda')
+        for name in refgold.REDUCE_OPS:
+            d_o = bf.empty(refgold.reduce_oshape(ci), 'f32', 'cuda')
             bf.reduce(d_a, d_o, name)
-            _check(ref.bfReduce(d_a.as_BFarray(), d_r.as_BFarray(), code))
-            _check(ref.bfStreamSynchronize())
-            ours, theirs = np.asarray(d_o.copy('system')), np.asarray(d_r.copy('system'))
+            ours = np.asarray(d_o.copy('system')).ravel()
+            ours = ours[refgold.sample_index(ours.size, 1000 * ci)]
+            theirs = gold[refgold.reduce_key(ci, name)]
             if name in ('sum', 'min', 'max', 'pwrsum'):
                 np.testing.assert_array_equal(ours, theirs, err_msg=str((shape, axis, n, name)))
             else:

@@ -5,9 +5,10 @@ Parity is pinned two ways:
   * tests/golden/ring_traces.json.gz -- scripts of calls with the answers the
     reference's unmodified src/ring_impl.cpp gave (tests/golden/make_ring_golden.py);
     replayed here call by call, no reference needed;
+  * longer random scripts (the same file, 'live'), recorded the same way;
   * live, when oracle/_ref/libbifrost_ref_ring.so is present (built by
-    oracle/ref_ring_build.sh; it travels to the GPU box): fresh random scripts
-    on both libraries.
+    oracle/ref_ring_build.sh): the stored traces are checked to be what the
+    reference does, and the threaded tests below run on it too.
 The remaining tests exercise what a single-threaded script cannot: blocking
 calls between threads, and rings in device memory (-m gpu).
 """
@@ -29,9 +30,9 @@ REF = rt.load_reference()
 needs_ref = pytest.mark.skipif(REF is None, reason='oracle/_ref/libbifrost_ref_ring.so not built')
 
 
-def golden_cases():
+def golden_cases(kind='cases'):
     with gzip.open(os.path.join(HERE, 'golden', 'ring_traces.json.gz')) as f:
-        return json.loads(f.read().decode())['cases']
+        return json.loads(f.read().decode())[kind]
 
 
 def assert_same_trace(script, want, got):
@@ -54,11 +55,12 @@ def test_golden_traces_are_what_the_reference_does():
     assert rt.replay(REF, case['script']) == case['trace']
 
 
-@needs_ref
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('seed', range(100, 112))
 def test_live_differential_against_the_reference_ring(seed):
-    script, want = rt.generate(REF, seed, 350)
+    """Scripts of 350 random steps, recorded on the reference's ring."""
+    case = {c['seed']: c for c in golden_cases('live')}[seed]
+    script, want = case['script'], case['trace']
     assert len(script) > 100
     assert_same_trace(script, want, rt.replay(OURS, script))
 

@@ -1,4 +1,4 @@
-"""One launch each of the fused spectrometer and the tcgen05 correlator for ncu
+"""One launch each of the fused spectrometer and the wgmma correlator for ncu
 captures (not a benchmark: numbers under ncu are never reported)."""
 import os
 import sys
@@ -52,7 +52,7 @@ if 'beamform' in which:
             ms = (time.perf_counter() - t0) * 100
             ops = 8.0 * nchan * nbeam * nin * ntime
             print(json.dumps(dict(op='a.b ci8 beamformer %dx%dx%d x%d chan' % (nbeam, nin, ntime, nchan),
-                                  path='simt' if env else 'tcgen05', ms=ms, TOPs=ops / ms / 1e9,
+                                  path='simt' if env else 'wgmma', ms=ms, TOPs=ops / ms / 1e9,
                                   out_GBps=nchan * nbeam * ntime * 8 / ms / 1e6)))
         os.environ.pop('BFB_LINALG_SIMT', None)
 print('done')
