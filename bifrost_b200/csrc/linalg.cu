@@ -9,7 +9,9 @@
 //   c[..., i, j] = alpha * sum_t conj(u[t][i]) * u[t][j] + beta * c[..., i, j]   for i >= j
 // and every element above the diagonal is left untouched
 // (python/bifrost/blocks/correlate.py:69, test/test_pipeline.py:258-298,
-// test/test_linalg.py:168-185).  Integer inputs accumulate exactly in int32.
+// test/test_linalg.py:168-185).  Integer inputs accumulate exactly in int32,
+// in time chunks short enough for that (TC_MAX_SUM_LEN below); every int8
+// value, -128 included, is used as it is.
 //
 // Two kernels:
 //  * corr_tc_kernel -- int8 wgmma tensor cores.  The interleaved complex
@@ -132,6 +134,18 @@ corr_simt_kernel(SimtParams P) {
 // the MMAs of slab k.
 enum { TC_KT = 64, TC_STAGES = 3, TC_TILE_BYTES = TC_KT * 128, TC_CONSUMERS = 256,
        TC_THREADS = TC_CONSUMERS + 32, TC_STAGE_BYTES = 3 * TC_TILE_BYTES };   // A | B0 | B1
+
+// Exactness bounds of the integer sums.  Every int8 value, -128 included, has
+// |x| <= 128, so a sum of L products of two int8 values is bounded by L·128².
+// One int32 wgmma accumulator (one Gram entry) is therefore exact for
+// L <= TC_MAX_SUM_LEN = 131071.  The sum of two such entries, bounded by
+// L·2·128², fits int32 for L <= PAIR_MAX_SUM_LEN = 65535: there the epilogues
+// combine in int32, beyond it in 64 bits (WIDE), and round to fp32 once.
+// corr_simt_kernel<int8_t, int> sums both products of a pair in int32, so one
+// pass of it is exact for L <= PAIR_MAX_SUM_LEN.  Longer correlations are
+// split along time (correlate()).
+constexpr long TC_MAX_SUM_LEN   = ((1L << 31) - 1) / (128L * 128L);
+constexpr long PAIR_MAX_SUM_LEN = ((1L << 31) - 1) / (2L * 128L * 128L);
 
 struct TcParams {
 	float2* c; long c_row, c_batch;      // float2 units
@@ -319,6 +333,14 @@ __device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtens
 	return true;
 }
 
+// a + b rounded once to fp32.  WIDE: the sum may leave the int32 range.  The
+// 64-bit conversion runs at a quarter of the 32-bit rate on sm_90, so sums
+// that cannot overflow (reduction length <= PAIR_MAX_SUM_LEN) use the 32-bit one.
+template<bool WIDE>
+__device__ __forceinline__ float sum_to_f32(int a, int b) {
+	return WIDE ? (float)((long long)a + b) : (float)(a + b);
+}
+
 // Fragment of column block h -> staging[64][65] (complex rows il, columns jl).
 // The wgmma accumulator holds, per thread, rows 64 g + 16 w + lane/4 (+8) and
 // column pairs (c, c+1), c = 8 j + 2 (lane%4): even rows 2i carry (G[2i][2j],
@@ -341,6 +363,7 @@ __device__ __forceinline__ void tc_stage(int const (&acc)[64], float2* staging, 
 		}
 }
 
+template<bool WIDE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 	extern __shared__ __align__(1024) unsigned char tc_smem[];
@@ -368,7 +391,7 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 		const int J = J0 + h;
 		// even lane: Re = G[2i][2j] + G[2i+1][2j+1]; odd lane: Im = G[2i][2j+1] - G[2i+1][2j]
 		tc_stage(acc[h], staging, [](int mine0, int other1, int par) {
-			return (float)(par ? (other1 - mine0) : (mine0 + other1)); });
+			return sum_to_f32<WIDE>(par ? other1 : mine0, par ? -mine0 : other1); });
 		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
 		for( int idx = threadIdx.x; idx < 64 * 64; idx += TC_CONSUMERS ) {
 			const int il2 = idx >> 6, jl2 = idx & 63;
@@ -406,9 +429,10 @@ struct AbTcParams {
 	int   njj;                           // column-block pairs per row block
 	int   a_batched;                     // 0: one At for every batch entry
 	float alpha, beta;
-	float s_re, s_01, s_10;              // Re = G00 + s_re G11, Im = s_01 G01 + s_10 G10
+	int   s_re, s_01, s_10;              // Re = G00 + s_re G11, Im = s_01 G01 + s_10 G10 (signs)
 };
 
+template<bool WIDE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 ab_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, AbTcParams P) {
 	extern __shared__ __align__(1024) unsigned char tc_smem[];
@@ -423,14 +447,16 @@ ab_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
 	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
 	float2* staging = (float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
 	float2* cb = P.c + (long)batch * P.c_batch;
-	const float s_re = P.s_re, s_01 = P.s_01, s_10 = P.s_10;
+	const int s_re = P.s_re, s_01 = P.s_01, s_10 = P.s_10;
 #pragma unroll
 	for( int h=0; h<2; ++h ) {
 		if( h >= nb ) break;
 		const int J = J0 + h;
-		// even row 2m: (G00, G01); odd row 2m+1: (G10, G11); the partner's second entry
+		// even row 2m: (G00, G01); odd row 2m+1: (G10, G11); the partner's second entry.
+		// Combined exactly and rounded once: converting each entry to fp32 first
+		// loses the exact sum past 2^24, badly so when the terms cancel.
 		tc_stage(acc[h], staging, [=](int mine0, int other1, int par) {
-			return par ? (s_01 * (float)other1 + s_10 * (float)mine0) : ((float)mine0 + s_re * (float)other1); });
+			return sum_to_f32<WIDE>(par ? s_01 * other1 : mine0, par ? s_10 * mine0 : s_re * other1); });
 		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
 		for( int idx = threadIdx.x; idx < 64 * 64; idx += TC_CONSUMERS ) {
 			const int il2 = idx >> 6, jl2 = idx & 63;
@@ -518,8 +544,7 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 	for( int d=0; d<nbdim; ++d ) if( d != kdim ) nouter *= bshape[d];
 	bool tc_ok = utype == BF_DTYPE_CI8 && stride_i == 2 && stride_t % 16 == 0 &&
 	             (kb == 1 || (kb_ustr % 16 == 0 && kb_ustr >= 16)) && n >= 16 && ntime >= 1 &&
-	             ntime * 2L * 127 * 127 < (1L << 31) && get_encode_fn() != nullptr &&
-	             getenv("BFB_LINALG_SIMT") == nullptr;
+	             get_encode_fn() != nullptr && getenv("BFB_LINALG_SIMT") == nullptr;
 	for( long o=0; o<nouter; ++o ) {
 		long rem = o, uoff = 0, coff = 0;
 		for( int d=nbdim-1; d>=0; --d ) {
@@ -530,50 +555,60 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 		const char* ub = (const char*)udata + uoff;
 		float2* cb = (float2*)((char*)cdata + coff);
 		bool use_tc = tc_ok && ((uintptr_t)ub % 16 == 0);
-		if( use_tc ) {
-			CUtensorMap tmap;
-			cuuint64_t gdim[3] = {(cuuint64_t)(2 * n), (cuuint64_t)ntime, (cuuint64_t)kb};
-			cuuint64_t gstr[2] = {(cuuint64_t)stride_t, (cuuint64_t)(kb > 1 ? kb_ustr : stride_t * ntime)};
-			if( gstr[1] % 16 ) gstr[1] = round_up<cuuint64_t>(gstr[1], 16);
-			cuuint32_t box[3] = {128, TC_KT, 1};
-			cuuint32_t estr[3] = {1, 1, 1};
-			CUresult res = get_encode_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ub, gdim, gstr,
-			                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-			                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-			if( res != CUDA_SUCCESS ) use_tc = false;
+		// Integer sums are exact only up to a bounded length (TC_MAX_SUM_LEN,
+		// PAIR_MAX_SUM_LEN), so a longer integration runs as consecutive
+		// time chunks: the first one applies (alpha, beta), the later ones add
+		// onto c with beta = 1.  A chunk base ub + t0·stride_t stays 16-byte
+		// aligned (stride_t % 16 == 0 on the TC path), so the path holds.
+		long t0 = 0;
+		do {
+			const long maxlen = use_tc ? TC_MAX_SUM_LEN : utype == BF_DTYPE_CI8 ? PAIR_MAX_SUM_LEN : ntime;
+			const long nt = std::min(maxlen, ntime - t0);
+			const char* ut = ub + t0 * stride_t;
+			const float beta_t = t0 == 0 ? (float)beta : 1.f;
 			if( use_tc ) {
+				CUtensorMap tmap;
+				cuuint64_t gdim[3] = {(cuuint64_t)(2 * n), (cuuint64_t)nt, (cuuint64_t)kb};
+				cuuint64_t gstr[2] = {(cuuint64_t)stride_t, (cuuint64_t)(kb > 1 ? kb_ustr : stride_t * nt)};
+				if( gstr[1] % 16 ) gstr[1] = round_up<cuuint64_t>(gstr[1], 16);
+				cuuint32_t box[3] = {128, TC_KT, 1};
+				cuuint32_t estr[3] = {1, 1, 1};
+				CUresult res = get_encode_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ut, gdim, gstr,
+				                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+				                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+				if( res != CUDA_SUCCESS ) { use_tc = false; continue; }      // this chunk again, on SIMT
 				TcParams P;
 				P.c = cb; P.c_row = c_row_bytes / 8; P.c_batch = kb_cstr / 8;
-				P.n = (int)n; P.ntime = (int)ntime;
+				P.n = (int)n; P.ntime = (int)nt;
 				int T = (int)div_up<long>(2 * n, 128);
 				P.ntile = 0;
 				for( int i=0; i<T; ++i ) P.ntile += i / 2 + 1;     // (row block, column-block pair) units
-				P.alpha = (float)alpha; P.beta = (float)beta; P.conj_u = conj_u;
+				P.alpha = (float)alpha; P.beta = beta_t; P.conj_u = conj_u;
 				const size_t smem = tc_smem_bytes();
-				BFB_CUDA(cudaFuncSetAttribute(corr_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+				auto kernel = nt > PAIR_MAX_SUM_LEN ? corr_tc_kernel<true> : corr_tc_kernel<false>;
+				BFB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
 				                              (int)smem), BF_STATUS_INTERNAL_ERROR);
 				dim3 grid(P.ntile, (unsigned)kb);
-				corr_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tmap, P);
-				count_launch();
-				BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
-				continue;
+				kernel<<<grid, TC_THREADS, smem, st>>>(tmap, P);
+			} else {
+				SimtParams S;
+				S.u = ut; S.stride_t = stride_t; S.stride_i = stride_i; S.stride_b = kb_ustr;
+				S.c = cb; S.c_row = c_row_bytes / 8; S.c_batch = kb_cstr / 8;
+				S.n = (int)n; S.ntime = (int)nt; S.nbatch = (int)kb;
+				S.alpha = (float)alpha; S.beta = beta_t; S.conj_u = conj_u;
+				int T = (int)div_up<long>(n, 32);
+				dim3 grid(T * (T + 1) / 2, (unsigned)kb);
+				switch( utype ) {
+				case BF_DTYPE_CI8:  corr_simt_kernel<int8_t, int><<<grid, 256, 0, st>>>(S); break;
+				case BF_DTYPE_CI16: corr_simt_kernel<int16_t, float><<<grid, 256, 0, st>>>(S); break;
+				case BF_DTYPE_CF32: corr_simt_kernel<float, float><<<grid, 256, 0, st>>>(S); break;
+				default: BFB_FAIL(BF_STATUS_UNSUPPORTED_DTYPE);
+				}
 			}
-		}
-		SimtParams S;
-		S.u = ub; S.stride_t = stride_t; S.stride_i = stride_i; S.stride_b = kb_ustr;
-		S.c = cb; S.c_row = c_row_bytes / 8; S.c_batch = kb_cstr / 8;
-		S.n = (int)n; S.ntime = (int)ntime; S.nbatch = (int)kb;
-		S.alpha = (float)alpha; S.beta = (float)beta; S.conj_u = conj_u;
-		int T = (int)div_up<long>(n, 32);
-		dim3 grid(T * (T + 1) / 2, (unsigned)kb);
-		switch( utype ) {
-		case BF_DTYPE_CI8:  corr_simt_kernel<int8_t, int><<<grid, 256, 0, st>>>(S); break;
-		case BF_DTYPE_CI16: corr_simt_kernel<int16_t, float><<<grid, 256, 0, st>>>(S); break;
-		case BF_DTYPE_CF32: corr_simt_kernel<float, float><<<grid, 256, 0, st>>>(S); break;
-		default: BFB_FAIL(BF_STATUS_UNSUPPORTED_DTYPE);
-		}
-		count_launch();
-		BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+			count_launch();
+			BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+			t0 += nt;
+		} while( t0 < ntime );
 	}
 	return BF_STATUS_SUCCESS;
 }
@@ -663,14 +698,14 @@ static bool ab_kind_ok(BFdtype t) {
 // The tensor-core form of the product, when the operands allow it (returns
 // false to leave the call to the SIMT kernel): ci8 x ci8 -> cf32, b rows
 // contiguous and 16-byte aligned (TMA), c rows contiguous, at most one batch
-// dimension, sums that fit int32.
+// dimension, K <= TC_MAX_SUM_LEN (exact int32 sums).
 static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFstatus* status) {
 	*status = BF_STATUS_SUCCESS;
 	if( getenv("BFB_LINALG_SIMT") || !get_encode_fn() ) return false;
 	if( P.a.kind != BF_DTYPE_CI8 || P.b.kind != BF_DTYPE_CI8 || P.c_kind != BF_DTYPE_CF32 ) return false;
 	if( P.nb > 1 || P.c_n != 8 || P.c_m % 8 || P.b.sm != 2 || P.b.sk % 16 || ((uintptr_t)P.b.p % 16) ) return false;
 	if( P.nb == 1 && (P.b.sb[0] % 16 || P.c_b[0] % 8 || P.b.sb[0] == 0) ) return false;
-	if( (long)P.K * 2 * 127 * 127 >= (1L << 31) || P.K < 1 || P.M < 1 || P.N < 8 ) return false;
+	if( P.K > TC_MAX_SUM_LEN || P.K < 1 || P.M < 1 || P.N < 8 ) return false;
 	cudaStream_t st = thread_stream();
 	// a^T, k slow: [batch][K][pitch]
 	const bool a_batched = P.nb == 1 && P.a.sb[0] != 0;
@@ -713,15 +748,16 @@ static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFsta
 	Q.a_batched = a_batched ? 1 : 0;
 	Q.alpha = (float)P.alpha; Q.beta = (float)P.beta;
 	const bool ca = P.a.conj != 0, cb = P.b.conj != 0;
-	Q.s_re = (ca != cb) ? 1.f : -1.f;
-	Q.s_01 = cb ? -1.f : 1.f;
-	Q.s_10 = ca ? -1.f : 1.f;
+	Q.s_re = (ca != cb) ? 1 : -1;
+	Q.s_01 = cb ? -1 : 1;
+	Q.s_10 = ca ? -1 : 1;
 	const size_t smem = tc_smem_bytes();
-	if( cudaFuncSetAttribute(ab_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
+	auto kernel = P.K > PAIR_MAX_SUM_LEN ? ab_tc_kernel<true> : ab_tc_kernel<false>;
+	if( cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
 		*status = BF_STATUS_INTERNAL_ERROR; return true;
 	}
 	dim3 grid((unsigned)(div_up<int>(P.M, 64) * Q.njj), (unsigned)nbatch);
-	ab_tc_kernel<<<grid, TC_THREADS, smem, st>>>(ta, tb, Q);
+	kernel<<<grid, TC_THREADS, smem, st>>>(ta, tb, Q);
 	count_launch();
 	if( cudaGetLastError() != cudaSuccess ) *status = BF_STATUS_INTERNAL_ERROR;
 	return true;

@@ -57,7 +57,8 @@ def run_bhb(x_tcn, beta=0.0, alpha=1.0, c0=None, perm=(1, 0, 2)):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("ntime,nchan,n", [(512, 4, 512), (100, 3, 128), (64, 2, 64), (1000, 1, 72),
-                                           (8, 5, 200), (33, 2, 16), (129, 1, 136)])
+                                           (8, 5, 200), (33, 2, 16), (129, 1, 136), (65, 1, 704),
+                                           (193, 2, 1024)])
 def test_tensor_core_path_is_integer_exact(ntime, nchan, n):
     rng = np.random.default_rng(ntime + n)
     x = rand_ci8(rng, (ntime, nchan, n))
