@@ -29,8 +29,8 @@
 //    stride-R scatter of the first stage and the unit-stride later stages are
 //    bank-conflict free.
 //  * any other n <= 8192: direct O(n^2) DFT from shared memory with an exact
-//    twiddle table (correct, not fast; covers the odd sizes of the reference's
-//    tests).
+//    twiddle table and sums kept in double (correct, not fast; covers the odd
+//    sizes of the reference's tests).
 //  * n = 2^k > 8192 (c2c): four-step, n = n1*n2, two passes of the same kernel
 //    through the plan's workspace with the inter-pass twiddle W_n^(k1*c2)
 //    applied on store.
@@ -403,15 +403,18 @@ fft_pass_kernel(const __grid_constant__ FftPass<T> P) {
 			fft_line_offsets(P, L, ioff, ooff, twc);
 			const T* lre = sre + (size_t)b * n;
 			const T* lim = sim + (size_t)b * n;
-			T ar = 0, ai = 0;
+			// double sums: an fp32 running sum over n terms drifts like sqrt(n)
+			// and passes 1e-5 of the output rms near n = 8192
+			double ar = 0, ai = 0;
 			int m = 0;
 			for( int e=0; e<n; ++e ) {
 				const T* w = P.twid + 2 * (size_t)m;
-				ar += lre[e] * w[0] - lim[e] * w[1];
-				ai += lre[e] * w[1] + lim[e] * w[0];
+				const double xr = lre[e], xi = lim[e];
+				ar += xr * w[0] - xi * w[1];
+				ai += xr * w[1] + xi * w[0];
 				m += o; if( m >= n ) m -= n;
 			}
-			fft_store(P, (char*)P.out + ooff, o, ar, ai, twc);
+			fft_store(P, (char*)P.out + ooff, o, (T)ar, (T)ai, twc);
 		}
 	}
 }
@@ -816,10 +819,12 @@ BFstatus run_pass(BFfft_impl* plan, int ndim, const long* batch_shape, int axis,
 			return BF_STATUS_SUCCESS;
 		}
 	}
+	// The fast kernels index the line as a forward, unit-stride array of
+	// elements: a reversed axis (stride -isize_in) goes to fft_pass_kernel.
 	if( sizeof(T) == 4 && n >= 256 && n <= 4096 && is_pow2(n) && !in_real && !in_herm && !out_real && n_out == n && !post_tw &&
-	    shift != 3 && !P.b_fast_in && (!P.b_fast_out || out.strides[axis] % 8 == 0) && out.strides[axis] > 0 &&
+	    shift != 3 && in.strides[axis] == isize_in && (!P.b_fast_out || out.strides[axis] % 8 == 0) && out.strides[axis] > 0 &&
 	    (in.kind == FK_CF32 || in.kind == FK_CI8 || in.kind == FK_CI16) &&
-	    (uintptr_t)in.data % isize_in == 0 ) {
+	    (uintptr_t)in.data % isize_in == 0 && (uintptr_t)out.data % 8 == 0 ) {
 		bool aligned = true;
 		for( int d=0; d<P.nouter; ++d ) aligned = aligned && (P.oistr[d] % isize_in == 0) && (P.oostr[d] % 8 == 0);
 		if( aligned ) {

@@ -18,6 +18,7 @@ import pytest
 import bifrost_b200 as bf
 from bifrost_b200.libbifrost import _bf
 from bifrost_b200.linalg import LinAlg
+from kernel_trace import device_kernels
 from oracle import linalg as olinalg
 
 pytestmark = pytest.mark.gpu
@@ -27,39 +28,6 @@ CI16 = bf.DataType('ci16').as_numpy_dtype()
 
 
 # ------------------------------------------------------------------ helpers
-def device_kernels(fn, reset=None, attempts=5):
-    """Names of the device kernels that `fn` ran, in execution order.
-
-    A session counts only if it recorded exactly as many kernels as the
-    library launched (bf.launch_count()).  Now and then a profiler session
-    misses some or all of the device activity; then `reset` (if given) puts
-    the operands back and `fn` runs again in a new session, up to `attempts`
-    times.  If no session records every launch the helper fails: a path
-    check must never pass vacuously."""
-    import torch
-    from torch.autograd import DeviceType
-    from torch.profiler import ProfilerActivity, profile
-    seen = []
-    for _ in range(attempts):
-        if reset is not None:
-            reset()
-        torch.cuda.synchronize()
-        before = bf.launch_count()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            bf.device.stream_synchronize()
-            torch.cuda.synchronize()
-        launched = bf.launch_count() - before
-        events = sorted((e.start_ns(), e.name()) for e in prof.profiler.kineto_results.events()
-                        if e.device_type() == DeviceType.CUDA)
-        names = [name for _, name in events if not name.startswith(('Memcpy', 'Memset'))]
-        if names and len(names) == launched:
-            return names
-        seen.append((launched, len(names)))
-    raise AssertionError("torch.profiler did not record every kernel launch "
-                         "(launched, recorded per session: %s)" % seen)
-
-
 def corr_paths(names):
     """'tc' / 'simt' for each correlator kernel among `names`."""
     return ['tc' if 'corr_tc_kernel' in k else 'simt' for k in names if 'corr_tc_kernel' in k or 'corr_simt_kernel' in k]
