@@ -13,7 +13,7 @@ from bifrost_b200.DataType import DataType
 from bifrost_b200.Space import Space
 from bifrost_b200.ndarray import (ndarray, asarray, empty, zeros, empty_like,
                                   zeros_like, copy_array, memset_array)
-from bifrost_b200 import fdmt, fft, linalg
+from bifrost_b200 import fdmt, fft, linalg, visibilities
 from bifrost_b200.reduce import reduce
 from bifrost_b200.transpose import transpose
 from bifrost_b200.unpack import unpack

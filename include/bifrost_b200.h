@@ -307,6 +307,22 @@ BFstatus bfAccumulate(BFarray const* a, BFarray const* b, double beta);
 BFstatus bfSpectrometerFused(BFarray const* in, BFarray const* out,
                              int nfft, int f_avg, double beta);
 
+/* Correlator output conversions (blocks/convert_visibilities.py).  cf32 in
+ * and out, device space, out-of-place (in and out byte ranges must not
+ * overlap).  C[r][s] is the matrix over r = 2*station + pol; only r >= s is
+ * read.  Leading batch dims may have any positive stride; the innermost axis
+ * is unit stride and every other stride a positive multiple of 8 bytes.
+ * FillHermitian: [..., n, n] -> [..., n, n]; out[r][s] = in[r][s] for r >= s,
+ *   conj(in[s][r]) for r < s.
+ * ToStorage: [..., nchan, nstand, 2, nstand, 2] -> [..., nbaseline, nchan, 4]
+ *   with baseline b = i(i+1)/2 + j (i >= j) and Stokes I = xx + yy,
+ *   Q = xx - yy, U = xy + yx, V = i(xy - yx); xy = conj(yx) when i == j.
+ * FromStorage: the inverse, out fully written: xx = (I+Q)/2, yy = (I-Q)/2,
+ *   xy = (U - iV)/2, yx = (U + iV)/2, the upper triangle mirrored. */
+BFstatus bfVisibilitiesFillHermitian(BFarray const* in, BFarray const* out);
+BFstatus bfVisibilitiesToStorage(BFarray const* in, BFarray const* out);
+BFstatus bfVisibilitiesFromStorage(BFarray const* in, BFarray const* out);
+
 /* Host-only introspection of the FDMT plan bfFdmtInit would build (no device
  * needed).  step < 0: writes the number of steps to *nrow.  Otherwise writes
  * the row count of `step` to *nrow and, if rows != NULL, nrow triples

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -221,6 +221,36 @@ def main():
                    2 * ntime * nchan_c * n + 8 * nchan_c * n * (n + 1) / 2, rms,
                    TFLOPs=round(flops / ms / 1e9, 1))
             del d_x, d_c
+
+    if 'visibilities' in ops:
+        # BASELINE config 4 correlator output, one frame: 512 chan x (256 stations x 2 pols)^2 cf32.
+        # Compulsory bytes: the lower triangle read (or the storage tensor) plus the output
+        # written.  copy_* is a device-to-device copy moving the same bytes (half read, half
+        # written), timed in the same run: the practical ceiling for a streaming kernel.
+        nchan_v, nstand = 512, 256
+        n, nb = 2 * nstand, nstand * (nstand + 1) // 2
+        low = 8 * nchan_v * n * (n + 1) // 2
+        full, sto = 8 * nchan_v * n * n, 32 * nchan_v * nb
+        c = rng.standard_normal(size=(nchan_v, n, n), dtype=np.float32).astype(np.complex64)
+        d_m = bf.asarray(c, space='cuda')
+        del c
+        d_f = bf.empty((nchan_v, n, n), 'cf32', 'cuda')
+        d_s = bf.empty((nb, nchan_v, 4), 'cf32', 'cuda')
+        m6 = d_m.reshape(nchan_v, nstand, 2, nstand, 2)
+        f6 = d_f.reshape(nchan_v, nstand, 2, nstand, 2)
+        buf = torch.empty(full, dtype=torch.uint8, device='cuda')
+        dst = torch.empty_like(buf)
+        for name, fn, nbytes in (
+                ('fill_hermitian', lambda: bf.visibilities.fill_hermitian(d_m, d_f), low + full),
+                ('to_storage', lambda: bf.visibilities.to_storage(m6, d_s), low + sto),
+                ('from_storage', lambda: bf.visibilities.from_storage(d_s, f6), sto + full)):
+            ms = timeit(fn, nrep=20, stream=stream)
+            half = nbytes // 2
+            cms = timeit(lambda: dst[:half].copy_(buf[:half]), nrep=20, stream=stream)
+            report('visibilities.%s nchan=%d nstand=%d' % (name, nchan_v, nstand), ms, nbytes,
+                   copy_ms=round(cms, 4), copy_GBps=round(nbytes / cms / 1e6, 1),
+                   of_copy=round(cms / ms, 3))
+        del d_m, d_f, d_s, buf, dst
 
 
 if __name__ == '__main__':
