@@ -11,6 +11,7 @@ from bifrost_b200.blocks.accumulate import accumulate, AccumulateBlock
 from bifrost_b200.blocks.fdmt import fdmt, FdmtBlock
 from bifrost_b200.blocks.correlate import correlate, CorrelateBlock
 from bifrost_b200.blocks.convert_visibilities import convert_visibilities, ConvertVisibilitiesBlock
+from bifrost_b200.blocks.beamform import beamform, BeamformBlock
 from bifrost_b200.blocks.unpack import unpack, UnpackBlock
 from bifrost_b200.blocks.quantize import quantize, QuantizeBlock
 from bifrost_b200.blocks.guppi_raw import read_guppi_raw, GuppiRawSourceBlock

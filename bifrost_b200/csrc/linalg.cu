@@ -30,6 +30,7 @@
 //    cannot describe (strides not multiples of 16 B, a.a^H form, ci16/cf32).
 #include "core.hpp"
 #include "shape.hpp"
+#include "beamform.hpp"
 
 #include <cuda.h>
 #include <algorithm>
@@ -619,9 +620,10 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 // General product c = alpha a.b + beta c (reference: bfMatMul_ab,
 // src/linalg.cu:479-637, cuBLAS / the beamformer kernel there).  A plain tiled
 // SIMT GEMM with per-element loaders: any strides, conjugated views, and
-// ci8 / ci16 / cf32 / f32 (float accumulation) or f64 / cf64 (double) inputs.
-// It exists for API completeness (beamforming, reference test_linalg.py
-// matmul_ab cases); the tensor-core work of this library is the correlator.
+// ci4 / ci8 / ci16 / cf32 / f32 (float accumulation) or f64 / cf64 (double)
+// inputs.  It exists for API completeness (reference test_linalg.py matmul_ab
+// cases) and as the reference the beamformer (beamform.cu) is tested against;
+// the hot paths are the beamformer and the tensor-core correlator.
 namespace bfb {
 
 struct AbOperand { const char* p; long sm, sk, sb[BF_MAX_DIMS]; int kind, conj; };   // kind: BFdtype
@@ -635,6 +637,8 @@ struct AbParams {
 template<typename R>
 __device__ __forceinline__ void ab_load(const char* p, int kind, int conj, R& re, R& im) {
 	switch( kind ) {
+	case BF_DTYPE_CI4:  { signed char v = *(const signed char*)p;        // high nibble real
+	                      re = v >> 4; im = (signed char)(v << 4) >> 4; break; }
 	case BF_DTYPE_CI8:  { char2  v = *(const char2*)p;   re = v.x; im = v.y; break; }
 	case BF_DTYPE_CI16: { short2 v = *(const short2*)p;  re = v.x; im = v.y; break; }
 	case BF_DTYPE_CF32: { float2 v = *(const float2*)p;  re = v.x; im = v.y; break; }
@@ -691,7 +695,7 @@ matmul_ab_kernel(AbParams P) {
 }
 
 static bool ab_kind_ok(BFdtype t) {
-	return t == BF_DTYPE_CI8 || t == BF_DTYPE_CI16 || t == BF_DTYPE_CF32 || t == BF_DTYPE_CF64 ||
+	return t == BF_DTYPE_CI4 || t == BF_DTYPE_CI8 || t == BF_DTYPE_CI16 || t == BF_DTYPE_CF32 || t == BF_DTYPE_CF64 ||
 	       t == BF_DTYPE_F32 || t == BF_DTYPE_F64 || t == BF_DTYPE_I8;
 }
 
@@ -763,6 +767,31 @@ static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFsta
 	return true;
 }
 
+// The beamformer (beamform.cu), when the operands allow it (returns false to
+// leave the call to the other kernels): cf32 / ci16 weights a times ci4 / ci8
+// voltages b into cf32, unit stride along K in both, 8-byte multiple C strides.
+static bool matmul_ab_beamform(AbParams const& P, long nbatch, BFstatus* status) {
+	if( getenv("BFB_LINALG_SIMT") ) return false;
+	const long wsz = P.a.kind == BF_DTYPE_CF32 ? 8 : P.a.kind == BF_DTYPE_CI16 ? 4 : 0;
+	const long xsz = P.b.kind == BF_DTYPE_CI8 ? 2 : P.b.kind == BF_DTYPE_CI4 ? 1 : 0;
+	if( !wsz || !xsz || P.c_kind != BF_DTYPE_CF32 || P.a.sk != wsz || P.b.sk != xsz || P.K < 1 ) return false;
+	if( P.c_m % 8 || P.c_n % 8 || (uintptr_t)P.c % 8 || (uintptr_t)P.a.p % wsz || P.a.sm % wsz ) return false;
+	BeamformOperands op;
+	for( int d=0; d<P.nb; ++d ) {
+		if( P.c_b[d] % 8 || P.a.sb[d] % wsz ) return false;
+		op.w_b[d] = P.a.sb[d]; op.x_b[d] = P.b.sb[d]; op.c_b[d] = P.c_b[d]; op.bshape[d] = P.bshape[d];
+	}
+	op.wtype = (BFdtype)P.a.kind; op.xtype = (BFdtype)P.b.kind;
+	op.w = P.a.p; op.w_beam = P.a.sm; op.conj_w = P.a.conj;
+	op.x = P.b.p; op.x_time = P.b.sm; op.conj_x = P.b.conj;
+	op.c = P.c; op.c_beam = P.c_m; op.c_time = P.c_n;
+	op.nb = P.nb; op.nbatch = nbatch;
+	op.nbeam = P.M; op.ntime = P.N; op.K = P.K;
+	op.alpha = P.alpha; op.beta = P.beta;
+	*status = beamform_launch(op, thread_stream());
+	return true;
+}
+
 static BFstatus matmul_ab(BFlinalg_impl* handle, double alpha, BFarray const* a, BFarray const* b, double beta, BFarray const* c) {
 	BFB_ASSERT(space_on_device(a->space) && space_on_device(b->space), BF_STATUS_UNSUPPORTED_SPACE);
 	int nd = c->ndim;
@@ -798,6 +827,7 @@ static BFstatus matmul_ab(BFlinalg_impl* handle, double alpha, BFarray const* a,
 	BFB_ASSERT(nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
 	{
 		BFstatus tcs = BF_STATUS_SUCCESS;
+		if( matmul_ab_beamform(P, nbatch, &tcs) ) return tcs;
 		if( matmul_ab_tc(handle, P, nbatch, &tcs) ) return tcs;
 	}
 	dim3 grid((unsigned)div_up<int>(P.N, 16), (unsigned)div_up<int>(P.M, 16), (unsigned)nbatch);

@@ -242,8 +242,13 @@ BFstatus bfFftDestroy(BFfft plan);
  * LinAlg                              (ref: src/bifrost/linalg.h:43-54)
  * c = alpha*a.b + beta*c;  b==NULL: a.a^H;  a==NULL: b^H.b.
  * The a.a^H / b^H.b forms write the lower triangle only (wgmma int8 path for
- * ci8).  a.b is a general strided SIMT product (ci8/ci16/cf32/f32 with float
- * accumulation, f64/cf64 with double; conjugated views honoured).
+ * ci8).  a.b with cf32/ci16 weights a and ci4/ci8 voltages b, both unit
+ * stride along K, into cf32 (the beamformer layout) runs the sm_90a
+ * beamformer (csrc/beamform.cu: any nbeam, K and ntime, fixed k summation
+ * order).  Every other a.b is a general strided SIMT product (ci4/ci8/ci16/
+ * cf32/f32 with float accumulation, f64/cf64 with double; conjugated views
+ * honoured; ci4 is high nibble real).  BFB_LINALG_SIMT=1 forces the SIMT
+ * products.
  * ------------------------------------------------------------------ */
 typedef struct BFlinalg_impl* BFlinalg;
 

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -251,6 +251,71 @@ def main():
                    copy_ms=round(cms, 4), copy_GBps=round(nbytes / cms / 1e6, 1),
                    of_copy=round(cms / ms, 3))
         del d_m, d_f, d_s, buf, dst
+
+    if 'beamform' in ops:
+        bench_beamform(stream, ref, rng)
+
+
+def bench_beamform(stream, ref, rng):
+    """The beamformer layout of bfLinAlgMatMul: 512 chan, K = 256 stations x 2
+    pols, ntime 4096, cf32 weights, ci8 / ci4 voltages.  Times the sm_90a kernel,
+    the generic kernel (BFB_LINALG_SIMT=1), the reference's kernel (nbeam <= 16,
+    ci8: its CI8 @ CF32 path) and a device copy of the voltage bytes.  Bounds:
+    compulsory bytes (voltages + weights + output) at 3.35 TB/s and 8 flops per
+    complex multiply-add at 67 TFLOP/s (H100 SXM data sheet, 700 W)."""
+    import subprocess
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({'op': 'beamform.device', 'gpu': q[0] if q else None}), flush=True)
+    nchan, K, ntime = 512, 512, 4096
+    for xk in ('ci8', 'ci4'):
+        vb = 2 if xk == 'ci8' else 1
+        raw = rng.integers(0, 256, size=(ntime, nchan, K * vb), dtype=np.uint8)
+        xnp = raw.view(bf.DataType(xk).as_numpy_dtype()).reshape(ntime, nchan, K)
+        d_x = bf.asarray(bf.ndarray(xnp, dtype=xk), space='cuda')
+        del raw, xnp
+        xv = d_x.transpose((1, 2, 0))
+        buf = torch.empty(ntime * nchan * K * vb, dtype=torch.uint8, device='cuda')
+        dst = torch.empty_like(buf)
+        cms = timeit(lambda: dst.copy_(buf), nrep=20, stream=stream)
+        del buf, dst
+        for nbeam in (1, 4, 16, 64):
+            if xk == 'ci4' and nbeam == 64:
+                continue
+            w = (rng.normal(size=(nchan, nbeam, K)) + 1j * rng.normal(size=(nchan, nbeam, K))).astype(np.complex64)
+            d_w = bf.asarray(w, space='cuda')
+            d_c = bf.zeros((nchan, nbeam, ntime), 'cf32', 'cuda')
+            la = bf.linalg.LinAlg()
+            ms = timeit(lambda: la.matmul(1, d_w, xv, 0, d_c), nrep=20, stream=stream)
+            got = np.asarray(d_c.copy('system'))
+            os.environ['BFB_LINALG_SIMT'] = '1'
+            try:
+                sms = timeit(lambda: la.matmul(1, d_w, xv, 0, d_c), nrep=3, nwarm=1, stream=stream)
+                simt = np.asarray(d_c.copy('system'))
+            finally:
+                del os.environ['BFB_LINALG_SIMT']
+            # sum_k |w_k| |x_k| <= 128 sqrt(2) sum_k |w_k|: each kernel is within 1e-6 of it
+            tol = 2e-6 * 128 * np.sqrt(2) * np.abs(w).sum(-1)[..., None]
+            agree = bool(np.all(np.abs(got - simt) <= tol))
+            rms = None
+            if ref is not None and nbeam <= 16 and xk == 'ci8':
+                rl = ctypes.c_void_p()
+                _check(ref.bfLinAlgCreate(ctypes.byref(rl)))
+                st = ref.bfLinAlgMatMul(rl, 1.0, d_w.as_BFarray(), xv.as_BFarray(), 0.0, d_c.as_BFarray())
+                if st == 0:
+                    rms = timeit(lambda: ref.bfLinAlgMatMul(rl, 1.0, d_w.as_BFarray(), xv.as_BFarray(), 0.0,
+                                                            d_c.as_BFarray()), nrep=3, nwarm=1, stream=stream)
+                ref.bfLinAlgDestroy(rl)
+            nbytes = ntime * nchan * K * vb + nchan * nbeam * K * 8 + nchan * nbeam * ntime * 8
+            flops = 8.0 * nchan * nbeam * K * ntime
+            t_hbm, t_fp = nbytes / 3.35e12 * 1e3, flops / 67e12 * 1e3
+            report('beamform %s x cf32 nbeam=%d nchan=%d K=%d ntime=%d' % (xk, nbeam, nchan, K, ntime), ms, nbytes,
+                   rms, TFLOPs=round(flops / ms / 1e9, 2), bound_by='HBM' if t_hbm >= t_fp else 'FP32',
+                   share_of_bound=round(max(t_hbm, t_fp) / ms, 3), simt_ms=round(sms, 4),
+                   speedup_vs_simt=round(sms / ms, 1), copy_ms=round(cms, 4), agrees_with_simt=agree,
+                   max_abs_diff_vs_simt=float(np.abs(got - simt).max()))
+            del d_w, d_c
+        del d_x
 
 
 if __name__ == '__main__':
