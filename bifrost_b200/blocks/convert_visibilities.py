@@ -39,6 +39,25 @@ def _nstand(nbaseline):
     return lo
 
 
+def matrix_to_storage_header(ohdr):
+    """Rewrites, in place, a copy of a matrix sequence header into the header
+    of its storage form (also the header of correlate(..., output='storage'))."""
+    otensor = ohdr['_tensor']
+    nchan, nstand, npol = otensor['shape'][1:4]
+    if npol != 2:
+        raise ValueError("The storage form needs npol = 2, got %i" % npol)
+    del ohdr['matrix_fill_mode']
+    otensor['shape'] = [-1, nstand * (nstand + 1) // 2, nchan, 4]
+    otensor['labels'] = list(STORAGE_AXES)
+    if 'scales' in otensor:
+        s = otensor['scales']
+        otensor['scales'] = [s[0], None, s[1], None]
+    if 'units' in otensor:
+        u = otensor['units']
+        otensor['units'] = [u[0], None, u[1], list(STOKES_UNITS)]
+    return ohdr
+
+
 class ConvertVisibilitiesBlock(TransformBlock):
     def __init__(self, iring, fmt, *args, **kwargs):
         super(ConvertVisibilitiesBlock, self).__init__(iring, *args, **kwargs)
@@ -67,17 +86,7 @@ class ConvertVisibilitiesBlock(TransformBlock):
             if self.ofmt == 'matrix':
                 ohdr['matrix_fill_mode'] = 'hermitian'
             elif self.ofmt == 'storage':
-                if npol != 2:
-                    raise ValueError("The storage form needs npol = 2, got %i" % npol)
-                del ohdr['matrix_fill_mode']
-                otensor['shape'] = [-1, nstand * (nstand + 1) // 2, nchan, 4]
-                otensor['labels'] = list(STORAGE_AXES)
-                if 'scales' in otensor:
-                    s = otensor['scales']
-                    otensor['scales'] = [s[0], None, s[1], None]
-                if 'units' in otensor:
-                    u = otensor['units']
-                    otensor['units'] = [u[0], None, u[1], list(STOKES_UNITS)]
+                matrix_to_storage_header(ohdr)
             else:
                 raise NotImplementedError("Unsupported conversion from matrix to %s" % self.ofmt)
         elif labels == STORAGE_AXES:

@@ -1,17 +1,29 @@
 """correlate block (same contract as python/bifrost/blocks/correlate.py:37-138;
-the data path is bfLinAlgMatMul(a=NULL, b=x): the int8 tensor-core correlator)."""
+the data path is bfLinAlgMatMul(a=NULL, b=x): the int8 tensor-core correlator).
+
+output='storage' (extension) emits what convert_visibilities(..., 'storage')
+would make of the matrix output, bit for bit and with the same header, from
+bfLinAlgCorrelateToStorage: one kernel per integration when an integration is
+one gulp."""
 from bifrost_b200.pipeline import TransformBlock
 from bifrost_b200.linalg import LinAlg
 from bifrost_b200.blocks import _header as H
+from bifrost_b200.blocks.convert_visibilities import matrix_to_storage_header
+from bifrost_b200 import visibilities
+from bifrost_b200.ndarray import empty
 
 _IN_AXES = ['time', 'freq', 'station', 'pol']
 
 
 class CorrelateBlock(TransformBlock):
-    def __init__(self, iring, nframe_per_integration, *args, **kwargs):
+    def __init__(self, iring, nframe_per_integration, output='matrix', *args, **kwargs):
         super(CorrelateBlock, self).__init__(iring, *args, **kwargs)
+        if output not in ('matrix', 'storage'):
+            raise ValueError("output must be 'matrix' or 'storage', got %r" % (output,))
         self.nframe_per_integration = nframe_per_integration
+        self.output = output
         self.linalg = LinAlg()
+        self._acc = None            # storage output over several gulps: C is summed here
 
     def define_valid_input_spaces(self):
         return ('cuda',)
@@ -39,6 +51,8 @@ class CorrelateBlock(TransformBlock):
         if self.nframe_per_integration % gulp:
             raise ValueError("gulp_nframe (%i) does not divide nframe_per_integration (%i)"
                              % (gulp, self.nframe_per_integration))
+        if self.output == 'storage':
+            matrix_to_storage_header(ohdr)
         return ohdr
 
     def _gulp(self, iseq):
@@ -48,19 +62,35 @@ class CorrelateBlock(TransformBlock):
     def on_data(self, ispan, ospan):
         idata, odata = ispan.data, ospan.data
         ntime, nchan, nstand, npol = idata.shape
+        n = nstand * npol
         # [time, freq, stand*pol] -> [freq, time, stand*pol] view; out [freq, n, n]
-        x = idata.reshape(ntime, nchan, nstand * npol).transpose(1, 0, 2)
-        c = odata.reshape(nchan, nstand * npol, nstand * npol)
-        self.linalg.matmul(1., None, x, 1. if self.nframe_integrated else 0., c)
+        x = idata.reshape(ntime, nchan, n).transpose(1, 0, 2)
+        first = self.nframe_integrated == 0
+        done = self.nframe_integrated + ispan.nframe == self.nframe_per_integration
+        if self.output == 'matrix':
+            self.linalg.matmul(1., None, x, 0. if first else 1., odata.reshape(nchan, n, n))
+        elif first and done:
+            self.linalg.correlate_to_storage(x, odata.reshape(odata.shape[1:]))
+        else:
+            # the matrix block's sum, in a private buffer: an output frame holds Stokes only
+            if self._acc is None or self._acc.shape != (nchan, n, n):
+                self._acc = empty((nchan, n, n), dtype='cf32', space='cuda')
+            self.linalg.matmul(1., None, x, 0. if first else 1., self._acc)
+            if done:
+                visibilities.to_storage(self._acc.reshape(nchan, nstand, npol, nstand, npol),
+                                        odata.reshape(odata.shape[1:]))
         self.nframe_integrated += ispan.nframe
         if self.nframe_integrated > self.nframe_per_integration:
             raise RuntimeError("integration overran: gulp does not tile nframe_per_integration")
-        if self.nframe_integrated == self.nframe_per_integration:
+        if done:
             self.nframe_integrated = 0
             return 1
         return 0
 
 
 def correlate(iring, nframe_per_integration, *args, **kwargs):
-    """Cross-multiply ['time','freq','station','pol'] voltages into lower-triangular visibilities."""
+    """Cross-multiply ['time','freq','station','pol'] voltages into lower-triangular
+    visibilities ['time','freq','station_i','pol_i','station_j','pol_j'], or with
+    output='storage' into ['time','baseline','freq','stokes'] (the layout of
+    convert_visibilities(..., 'storage'), npol = 2)."""
     return CorrelateBlock(iring, nframe_per_integration, *args, **kwargs)

@@ -28,9 +28,15 @@
 //    below the diagonal are launched; diagonal tiles load one operand.
 //  * corr_simt_kernel -- shared-memory tiled SIMT fallback for layouts TMA
 //    cannot describe (strides not multiples of 16 B, a.a^H form, ci16/cf32).
+//
+// bfLinAlgCorrelateToStorage (extension) writes the b^H.b correlation straight
+// in the [baseline][chan][stokes] storage layout of bfVisibilitiesToStorage:
+// corr_storage_tc_kernel is corr_tc_kernel with a Stokes epilogue; every other
+// input runs the matrix correlator into a workspace and then the storage kernel.
 #include "core.hpp"
 #include "shape.hpp"
 #include "beamform.hpp"
+#include "stokes.cuh"
 
 #include <cuda.h>
 #include <algorithm>
@@ -411,6 +417,71 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 	}
 }
 
+// corr_tc_kernel (alpha 1, beta 0) followed by vis_to_storage_kernel, in one
+// pass: vis[b][chan][stokes] for baselines b = i (i + 1) / 2 + j, i >= j.
+// The 64 x 64 complex tile a column block leaves in staging is 32 stations i
+// (rows 2 il + p) by 32 stations j (columns 2 jl + q), so it holds the whole
+// 2 x 2 Jones block of each of its baselines.  Every entry is rounded as
+// corr_tc_kernel rounds it, and the Stokes steps are vis_to_storage_kernel's.
+struct StorageTcParams {
+	float2* vis; long s_base, s_chan;    // float2 units
+	int   nstand;
+	int   ntime;
+	int   conj_u;
+};
+
+template<bool WIDE>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	// Tiles fastest, as corr_tc_kernel: the CTAs resident together share a
+	// channel's voltages in L2.  Channel fastest (neighbouring 32 B pieces of
+	// the same baselines written together) measured 6-9 % slower (DESIGN.md §5).
+	const int batch = blockIdx.y;
+	int I = 0, rem = blockIdx.x;
+	while( rem >= I / 2 + 1 ) { rem -= I / 2 + 1; ++I; }
+	const int J0 = 2 * rem;
+	const int nb = (J0 + 1 <= I) ? 2 : 1;
+	const int alias = (J0 == I) ? 1 : (nb == 2 && J0 + 1 == I) ? 2 : 0;
+	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
+	int acc[2][64];
+	if( !tc_mainloop(tc_smem, &tmap, &tmap, 128 * I, batch, 128 * J0, batch, nb, alias, nk, acc) ) return;
+
+	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
+	const float2* staging = (const float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
+	float2* vc = P.vis + (long)batch * P.s_chan;
+#pragma unroll
+	for( int h=0; h<2; ++h ) {
+		if( h >= nb ) break;
+		const int J = J0 + h;
+		tc_stage(acc[h], (float2*)staging, [](int mine0, int other1, int par) {
+			return sum_to_f32<WIDE>(par ? other1 : mine0, par ? -mine0 : other1); });
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
+		// four neighbouring threads write the 32 B of one baseline
+		for( int e = threadIdx.x; e < 32 * 32 * 4; e += TC_CONSUMERS ) {
+			const int st = e & 3, jl = (e >> 2) & 31, il = e >> 7;
+			const long i = 32L * I + il, j = 32L * J + jl;
+			if( i < P.nstand && j <= i ) {
+				const float2* x = staging + (2 * il) * 65 + 2 * jl;       // xx, xy
+				const float2* y = x + 65;                                  // yx, yy
+				// the matrix entries exactly as corr_tc_kernel stores them
+				float2 xx = x[0], yx = y[0], yy = y[1];
+				float2 xy = (j == i) ? make_float2(0.f, 0.f) : x[1];
+				if( P.conj_u ) { xx.y = -xx.y; xy.y = -xy.y; yx.y = -yx.y; yy.y = -yy.y; }
+				float2 v;
+				if( st < 2 ) {
+					v = st == 0 ? cadd(xx, yy) : csub(xx, yy);
+				} else {
+					if( j == i ) xy = conj2(yx);
+					v = st == 2 ? cadd(xy, yx) : times_i(csub(xy, yx));
+				}
+				vc[(i * (i + 1) / 2 + j) * P.s_base + st] = v;
+			}
+		}
+		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
+	}
+}
+
 // ---------------------------------------------------------------------------
 // c = alpha a.b + beta c for ci8 operands on the tensor cores (the reference
 // hands this case to cublasCgemmEx with CUDA_C_8I inputs, src/linalg.cu:406-424;
@@ -522,10 +593,35 @@ struct BFlinalg_impl {
 	// a^T staging of the tensor-core a.b path (ci8), grown on demand
 	void*  at_buf = nullptr;
 	size_t at_size = 0;
-	~BFlinalg_impl() { if( at_buf ) cudaFree(at_buf); }
+	// cf32 [nchan][n][n] matrix of bfLinAlgCorrelateToStorage's workspace path, grown on demand
+	void*  vis_buf = nullptr;
+	size_t vis_size = 0;
+	~BFlinalg_impl() { if( at_buf ) cudaFree(at_buf); if( vis_buf ) cudaFree(vis_buf); }
 };
 
 namespace {
+
+// Whether the tensor-core correlator can read u(t, i) (kernel batch kb with
+// batch stride kb_ustr): ci8, interleaved complex bytes along i, 16-byte time
+// and batch strides that TMA can describe.  The base address is checked per
+// call (its alignment to 16 B).
+bool tc_layout_ok(BFdtype utype, long stride_t, long stride_i, long n, long ntime, long kb, long kb_ustr) {
+	return utype == BF_DTYPE_CI8 && stride_i == 2 && stride_t % 16 == 0 &&
+	       (kb == 1 || (kb_ustr % 16 == 0 && kb_ustr >= 16)) && n >= 16 && ntime >= 1 &&
+	       get_encode_fn() != nullptr && getenv("BFB_LINALG_SIMT") == nullptr;
+}
+
+// TMA map of nt time samples from ut: [kb][nt][2 n] bytes, [64 t][128 B] boxes.
+bool tc_encode_map(CUtensorMap* tmap, const char* ut, long n, long nt, long stride_t, long kb, long kb_ustr) {
+	cuuint64_t gdim[3] = {(cuuint64_t)(2 * n), (cuuint64_t)nt, (cuuint64_t)kb};
+	cuuint64_t gstr[2] = {(cuuint64_t)stride_t, (cuuint64_t)(kb > 1 ? kb_ustr : stride_t * nt)};
+	if( gstr[1] % 16 ) gstr[1] = round_up<cuuint64_t>(gstr[1], 16);
+	cuuint32_t box[3] = {128, TC_KT, 1};
+	cuuint32_t estr[3] = {1, 1, 1};
+	return get_encode_fn()(tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ut, gdim, gstr,
+	                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+	                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 // c[..,i,j] = alpha sum_t conj(u(t,i)) u(t,j) + beta c, lower triangle.
 // u(t,i) lives at data + t*stride_t + i*stride_i (+ batch offsets).
@@ -543,9 +639,7 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 	BFB_ASSERT(kb <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
 	long nouter = 1;
 	for( int d=0; d<nbdim; ++d ) if( d != kdim ) nouter *= bshape[d];
-	bool tc_ok = utype == BF_DTYPE_CI8 && stride_i == 2 && stride_t % 16 == 0 &&
-	             (kb == 1 || (kb_ustr % 16 == 0 && kb_ustr >= 16)) && n >= 16 && ntime >= 1 &&
-	             get_encode_fn() != nullptr && getenv("BFB_LINALG_SIMT") == nullptr;
+	bool tc_ok = tc_layout_ok(utype, stride_t, stride_i, n, ntime, kb, kb_ustr);
 	for( long o=0; o<nouter; ++o ) {
 		long rem = o, uoff = 0, coff = 0;
 		for( int d=nbdim-1; d>=0; --d ) {
@@ -569,15 +663,7 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 			const float beta_t = t0 == 0 ? (float)beta : 1.f;
 			if( use_tc ) {
 				CUtensorMap tmap;
-				cuuint64_t gdim[3] = {(cuuint64_t)(2 * n), (cuuint64_t)nt, (cuuint64_t)kb};
-				cuuint64_t gstr[2] = {(cuuint64_t)stride_t, (cuuint64_t)(kb > 1 ? kb_ustr : stride_t * nt)};
-				if( gstr[1] % 16 ) gstr[1] = round_up<cuuint64_t>(gstr[1], 16);
-				cuuint32_t box[3] = {128, TC_KT, 1};
-				cuuint32_t estr[3] = {1, 1, 1};
-				CUresult res = get_encode_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ut, gdim, gstr,
-				                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-				                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-				if( res != CUDA_SUCCESS ) { use_tc = false; continue; }      // this chunk again, on SIMT
+				if( !tc_encode_map(&tmap, ut, n, nt, stride_t, kb, kb_ustr) ) { use_tc = false; continue; }   // this chunk again, on SIMT
 				TcParams P;
 				P.c = cb; P.c_row = c_row_bytes / 8; P.c_batch = kb_cstr / 8;
 				P.n = (int)n; P.ntime = (int)nt;
@@ -891,6 +977,106 @@ BFstatus bfLinAlgMatMul(BFlinalg handle, double alpha, BFarray const* a, BFarray
 	}
 	BFB_TRY(return correlate(x->dtype, x->data, str_t, str_i, conj_u, n, ntime, nb, bshape, ustr, cstr,
 	                         c->data, c->strides[nd-2], alpha, beta, thread_stream()));
+}
+
+} // extern "C"
+
+namespace {
+
+// Byte range [lo, hi) an array touches.
+void array_bytes(BFarray const* a, uintptr_t* lo, uintptr_t* hi) {
+	long l = 0, h = dtype_nbyte(a->dtype);
+	for( int d=0; d<a->ndim; ++d ) {
+		long ext = (a->shape[d] - 1) * a->strides[d];
+		if( ext < 0 ) l += ext; else h += ext;
+	}
+	*lo = (uintptr_t)a->data + l;
+	*hi = (uintptr_t)a->data + h;
+}
+
+// The fused tensor-core pass, when x allows it (one launch); false leaves the
+// call to the workspace path.
+bool correlate_storage_tc(BFarray const* x, BFarray const* vis, BFstatus* status) {
+	const long nchan = x->shape[0], ntime = x->shape[1], n = x->shape[2];
+	const long kb_ustr = x->strides[0], stride_t = x->strides[1];
+	if( !tc_layout_ok(x->dtype, stride_t, x->strides[2], n, ntime, nchan, kb_ustr) ||
+	    ntime > TC_MAX_SUM_LEN || (uintptr_t)x->data % 16 ) return false;
+	CUtensorMap tmap;
+	if( !tc_encode_map(&tmap, (const char*)x->data, n, ntime, stride_t, nchan, kb_ustr) ) return false;
+	StorageTcParams P;
+	P.vis = (float2*)vis->data; P.s_base = vis->strides[0] / 8; P.s_chan = vis->strides[1] / 8;
+	P.nstand = (int)(n / 2); P.ntime = (int)ntime; P.conj_u = x->conjugated ? 1 : 0;
+	int T = (int)div_up<long>(2 * n, 128), ntile = 0;
+	for( int i=0; i<T; ++i ) ntile += i / 2 + 1;
+	const size_t smem = tc_smem_bytes();
+	auto kernel = ntime > PAIR_MAX_SUM_LEN ? corr_storage_tc_kernel<true> : corr_storage_tc_kernel<false>;
+	*status = BF_STATUS_SUCCESS;
+	if( cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
+		*status = BF_STATUS_INTERNAL_ERROR;
+		return true;
+	}
+	dim3 grid(ntile, (unsigned)nchan);
+	kernel<<<grid, TC_THREADS, smem, thread_stream()>>>(tmap, P);
+	count_launch();
+	if( cudaGetLastError() != cudaSuccess ) *status = BF_STATUS_INTERNAL_ERROR;
+	return true;
+}
+
+} // namespace
+
+extern "C" {
+
+BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis) {
+	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(x && vis, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(space_on_device(x->space) && space_on_device(vis->space), BF_STATUS_UNSUPPORTED_SPACE);
+	BFB_ASSERT(x->dtype == BF_DTYPE_CI8 || x->dtype == BF_DTYPE_CI16 || x->dtype == BF_DTYPE_CF32,
+	           BF_STATUS_UNSUPPORTED_DTYPE);
+	BFB_ASSERT(vis->dtype == BF_DTYPE_CF32, BF_STATUS_UNSUPPORTED_DTYPE);
+	BFB_ASSERT(!vis->conjugated, BF_STATUS_UNSUPPORTED);
+	BFB_ASSERT(x->ndim == 3 && vis->ndim == 3, BF_STATUS_INVALID_SHAPE);
+	const long nchan = x->shape[0], n = x->shape[2], nstand = n / 2;
+	BFB_ASSERT(n % 2 == 0, BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(vis->shape[0] == nstand * (nstand + 1) / 2 && vis->shape[1] == nchan && vis->shape[2] == 4,
+	           BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(nchan <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
+	// the storage side as bfVisibilitiesToStorage takes it
+	BFB_ASSERT(vis->strides[2] == 8 && (uintptr_t)vis->data % 8 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	for( int d=0; d<2; ++d )
+		BFB_ASSERT(vis->shape[d] == 1 || (vis->strides[d] > 0 && vis->strides[d] % 8 == 0),
+		           BF_STATUS_UNSUPPORTED_STRIDE);
+	if( nchan == 0 || nstand == 0 ) return BF_STATUS_SUCCESS;
+	{
+		uintptr_t xlo, xhi, vlo, vhi;
+		array_bytes(x, &xlo, &xhi);
+		array_bytes(vis, &vlo, &vhi);
+		BFB_ASSERT(array_numel(x) == 0 || xhi <= vlo || vhi <= xlo, BF_STATUS_INVALID_ARGUMENT);
+	}
+	BFstatus status;
+	if( correlate_storage_tc(x, vis, &status) ) return status;
+	// Workspace path: the matrix correlator, then the storage kernel -- the
+	// definition of this call, so its bits hold for every input.
+	const size_t need = (size_t)nchan * n * n * 8;
+	if( handle->vis_size < need ) {
+		cudaStreamSynchronize(thread_stream());
+		if( handle->vis_buf ) cudaFree(handle->vis_buf);
+		handle->vis_buf = nullptr; handle->vis_size = 0;
+		BFB_ASSERT(cudaMalloc(&handle->vis_buf, need) == cudaSuccess, BF_STATUS_MEM_ALLOC_FAILED);
+		handle->vis_size = need;
+	}
+	BFarray c;
+	std::memset(&c, 0, sizeof(c));
+	c.data = handle->vis_buf; c.space = BF_SPACE_CUDA; c.dtype = BF_DTYPE_CF32;
+	c.ndim = 3;
+	c.shape[0] = nchan; c.shape[1] = n; c.shape[2] = n;
+	c.strides[0] = n * n * 8; c.strides[1] = n * 8; c.strides[2] = 8;
+	status = bfLinAlgMatMul(handle, 1.0, nullptr, x, 0.0, &c);
+	if( status != BF_STATUS_SUCCESS ) return status;
+	BFarray m = c;                                   // [nchan][nstand][2][nstand][2]
+	m.ndim = 5;
+	const long shape[5] = {nchan, nstand, 2, nstand, 2}, strides[5] = {n * n * 8, 2 * n * 8, n * 8, 16, 8};
+	for( int d=0; d<5; ++d ) { m.shape[d] = shape[d]; m.strides[d] = strides[d]; }
+	return bfVisibilitiesToStorage(&m, vis);
 }
 
 } // extern "C"

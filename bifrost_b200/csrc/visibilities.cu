@@ -18,6 +18,7 @@
 // swaps, each rounded on its own (__fadd_rn / __fsub_rn / __fmul_rn), so the
 // results equal a float32 numpy restatement bit for bit (oracle/visibilities.py).
 #include "core.hpp"
+#include "stokes.cuh"
 
 namespace bfb {
 
@@ -40,12 +41,6 @@ __device__ __forceinline__ void batch_offsets(VisBatch const& B, long k, long* i
 	}
 	*io = i; *oo = o;
 }
-
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 conj2(float2 a)          { return make_float2(a.x, -a.y); }
-__device__ __forceinline__ float2 half2f(float2 a)         { return make_float2(__fmul_rn(0.5f, a.x), __fmul_rn(0.5f, a.y)); }
-__device__ __forceinline__ float2 times_i(float2 a)        { return make_float2(-a.y, a.x); }
 
 // ---------------------------------------------------------------- fill ----
 // One CTA per 32 x 32 tile on or below the diagonal.  An off-diagonal tile is

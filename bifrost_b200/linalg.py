@@ -17,3 +17,11 @@ class LinAlg(BifrostObject):
         _check(_bf.bfLinAlgMatMul(self.obj, alpha, a_array, b_array, beta,
                                   asarray(c).as_BFarray()))
         return c
+
+    def correlate_to_storage(self, x, vis):
+        """vis = the Stokes storage layout of x^H.x, written straight from the
+        correlator: x [nchan, ntime, 2 nstand] (ci8 / ci16 / cf32), vis
+        [nstand (nstand + 1) / 2, nchan, 4] cf32.  Bit for bit
+        visibilities.to_storage(matmul(1, None, x, 0, C)) with C [nchan, n, n]."""
+        _check(_bf.bfLinAlgCorrelateToStorage(self.obj, asarray(x).as_BFarray(), asarray(vis).as_BFarray()))
+        return vis

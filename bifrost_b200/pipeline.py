@@ -164,13 +164,20 @@ class Pipeline(object):
             -> detect('stokes') -> [merge_axes('freq', ...)] -> reduce('freq', f) -> accumulate(n)
         whose blocks were all created under fuse=True, each feeding only the next,
         is replaced by one SpectrometerBlock (one kernel launch per gulp,
-        bfSpectrometerFused) between the chain's input and output rings."""
+        bfSpectrometerFused) between the chain's input and output rings; and a
+        correlate(...) feeding only a convert_visibilities(..., 'storage'), both
+        created under fuse=True, by one correlate(..., output='storage')
+        (bfLinAlgCorrelateToStorage: the same output bits, one HBM pass fewer)."""
         from bifrost_b200.blocks.transpose import TransposeBlock
         from bifrost_b200.blocks.fft import FftBlock
         from bifrost_b200.blocks.detect import DetectBlock
         from bifrost_b200.blocks.reduce import ReduceBlock
         from bifrost_b200.blocks.accumulate import AccumulateBlock
         from bifrost_b200.blocks.spectrometer import SpectrometerBlock
+        from bifrost_b200.blocks.correlate import CorrelateBlock
+        from bifrost_b200.blocks.convert_visibilities import ConvertVisibilitiesBlock
+        if not hasattr(_tls, 'pipeline_stack'):
+            _tls.pipeline_stack = [Pipeline()]
 
         def only_consumer(ring, through_views=False):
             """The single block reading `ring` (optionally through one header view)."""
@@ -198,8 +205,6 @@ class Pipeline(object):
             if not (isinstance(a, AccumulateBlock) and a.fuse and a.dtype in (None, 'f32')):
                 continue
             iring, oring = t.irings[0], a.orings[0]
-            if not hasattr(_tls, 'pipeline_stack'):
-                _tls.pipeline_stack = [Pipeline()]
             _tls.pipeline_stack.append(self)
             try:
                 spec = SpectrometerBlock(iring, f_avg=r.specified_factor, n_int=a.nframe,
@@ -210,6 +215,25 @@ class Pipeline(object):
             spec.orings = [oring]
             oring.owner = spec
             for b in (t, f, d, r, a):
+                self.blocks.remove(b)
+
+        # correlate -> convert_visibilities('storage'): one CorrelateBlock(output='storage'),
+        # which writes the Stokes storage layout from the correlator (the same bits)
+        for c in [b for b in self.blocks if isinstance(b, CorrelateBlock) and b.fuse and b.output == 'matrix']:
+            v = only_consumer(c.orings[0])
+            if not (isinstance(v, ConvertVisibilitiesBlock) and v.fuse and v.ofmt == 'storage'):
+                continue
+            iring, oring = c.irings[0], v.orings[0]
+            _tls.pipeline_stack.append(self)
+            try:
+                corr = CorrelateBlock(iring, c.nframe_per_integration, output='storage',
+                                      gulp_nframe=c.gulp_nframe, gpu=c.gpu, core=c.core)
+            finally:
+                _tls.pipeline_stack.pop()
+            iring.consumers.remove(c)
+            corr.orings = [oring]
+            oring.owner = corr
+            for b in (c, v):
                 self.blocks.remove(b)
 
     def shutdown(self):

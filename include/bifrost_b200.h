@@ -328,6 +328,18 @@ BFstatus bfVisibilitiesFillHermitian(BFarray const* in, BFarray const* out);
 BFstatus bfVisibilitiesToStorage(BFarray const* in, BFarray const* out);
 BFstatus bfVisibilitiesFromStorage(BFarray const* in, BFarray const* out);
 
+/* Correlate straight into the storage layout: x is [nchan, ntime, 2*nstand]
+ * ci8 / ci16 / cf32 (the b of the b^H.b form of bfLinAlgMatMul, any strides
+ * it takes, conjugated views honoured), vis is [nbaseline, nchan, 4] cf32 as
+ * bfVisibilitiesToStorage writes it (padded baseline / channel strides, unit
+ * stride on Stokes).  vis is only written.  The result is that of
+ * bfLinAlgMatMul(handle, 1, NULL, x, 0, C) followed by
+ * bfVisibilitiesToStorage(C, vis), bit for bit.  ci8 inputs the tensor-core
+ * correlator takes in one pass (ntime <= 131071) run as one sm_90a kernel
+ * that writes the Stokes from its epilogue; every other input runs those two
+ * calls through a [nchan, n, n] workspace owned by the handle. */
+BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis);
+
 /* Host-only introspection of the FDMT plan bfFdmtInit would build (no device
  * needed).  step < 0: writes the number of steps to *nrow.  Otherwise writes
  * the row count of `step` to *nrow and, if rows != NULL, nrow triples

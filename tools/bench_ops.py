@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -255,6 +255,63 @@ def main():
     if 'beamform' in ops:
         bench_beamform(stream, ref, rng)
 
+    if 'correlate_storage' in ops:
+        bench_correlate_storage(stream, rng)
+
+
+def gpu_name():
+    """Card name, power limit and max SM clock, read in the same run as the timings."""
+    import subprocess
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    return q[0] if q else None
+
+
+def bench_correlate_storage(stream, rng, nrep=20):
+    """bfLinAlgCorrelateToStorage against the two calls it replaces
+    (bfLinAlgMatMul into a [chan, n, n] matrix, then bfVisibilitiesToStorage)
+    on BASELINE config 4: 512 chan, 256 stations x 2 pols, ci8.  The two are
+    timed alternately in the same loop, and their outputs compared bit for
+    bit.  HBM share: compulsory bytes (voltages read + Stokes written for the
+    fused call; + the lower triangle written and read back for the two calls)
+    at 3.35 TB/s (H100 SXM data sheet, 700 W) over the time."""
+    print(json.dumps({'op': 'correlate_storage.device', 'gpu': gpu_name()}), flush=True)
+    nchan, nstand = 512, 256
+    n, nb = 2 * nstand, nstand * (nstand + 1) // 2
+    la = bf.linalg.LinAlg()
+    d_c = bf.empty((nchan, n, n), 'cf32', 'cuda')
+    c6 = d_c.reshape(nchan, nstand, 2, nstand, 2)
+    d_f = bf.empty((nb, nchan, 4), 'cf32', 'cuda')
+    d_s = bf.empty((nb, nchan, 4), 'cf32', 'cuda')
+    fused = lambda: la.correlate_to_storage(xv, d_f)                                    # noqa: E731
+    two = lambda: (la.matmul(1, None, xv, 0, d_c), bf.visibilities.to_storage(c6, d_s))   # noqa: E731
+    for ntime in (512, 2048, 8192):
+        raw = rng.integers(-128, 128, size=(ntime, nchan, n, 2), dtype=np.int8)
+        d_x = bf.asarray(raw.view(bf.DataType('ci8').as_numpy_dtype()).reshape(ntime, nchan, n), space='cuda')
+        del raw
+        xv = d_x.transpose(1, 0, 2)                   # [chan, time, stand*pol] view of the ring frame
+        for fn in (fused, two, fused, two):
+            fn()
+        torch.cuda.synchronize()
+        times = {'fused': [], 'two': []}
+        for _ in range(nrep):
+            for key, fn in (('fused', fused), ('two', two)):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1))
+        identical = bool(np.array_equal(np.asarray(d_f.copy('system')).view(np.uint64),
+                                        np.asarray(d_s.copy('system')).view(np.uint64)))
+        ms, two_ms = float(np.median(times['fused'])), float(np.median(times['two']))
+        vin, vout, low = 2 * ntime * nchan * n, 32 * nchan * nb, 8 * nchan * n * (n + 1) // 2
+        report('correlate_storage ci8 ntime=%d nstand=%d nchan=%d' % (ntime, nstand, nchan), ms, vin + vout,
+               hbm_share=round((vin + vout) / 3.35e12 * 1e3 / ms, 3), two_call_ms=round(two_ms, 4),
+               two_call_hbm_share=round((vin + 2 * low + vout) / 3.35e12 * 1e3 / two_ms, 3),
+               speedup_vs_two_calls=round(two_ms / ms, 3), identical=identical)
+        del d_x, xv
+
 
 def bench_beamform(stream, ref, rng):
     """The beamformer layout of bfLinAlgMatMul: 512 chan, K = 256 stations x 2
@@ -263,10 +320,7 @@ def bench_beamform(stream, ref, rng):
     ci8: its CI8 @ CF32 path) and a device copy of the voltage bytes.  Bounds:
     compulsory bytes (voltages + weights + output) at 3.35 TB/s and 8 flops per
     complex multiply-add at 67 TFLOP/s (H100 SXM data sheet, 700 W)."""
-    import subprocess
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    print(json.dumps({'op': 'beamform.device', 'gpu': q[0] if q else None}), flush=True)
+    print(json.dumps({'op': 'beamform.device', 'gpu': gpu_name()}), flush=True)
     nchan, K, ntime = 512, 512, 4096
     for xk in ('ci8', 'ci4'):
         vb = 2 if xk == 'ci8' else 1
