@@ -1,5 +1,6 @@
 """correlate block (same contract as python/bifrost/blocks/correlate.py:37-138;
-the data path is bfLinAlgMatMul(a=NULL, b=x): the int8 tensor-core correlator).
+the data path is bfLinAlgMatMul(a=NULL, b=x), or bfLinAlgCorrelateCi4 for ci4:
+the int8 tensor-core correlator).
 
 output='storage' (extension) emits what convert_visibilities(..., 'storage')
 would make of the matrix output, bit for bit and with the same header, from
@@ -92,5 +93,8 @@ def correlate(iring, nframe_per_integration, *args, **kwargs):
     """Cross-multiply ['time','freq','station','pol'] voltages into lower-triangular
     visibilities ['time','freq','station_i','pol_i','station_j','pol_j'], or with
     output='storage' into ['time','baseline','freq','stokes'] (the layout of
-    convert_visibilities(..., 'storage'), npol = 2)."""
+    convert_visibilities(..., 'storage'), npol = 2).  The voltages may be ci4
+    (high nibble real), ci8, ci16 or cf32; ci4 gives the bytes of the same
+    pipeline on ci8 with the same values, without an unpack pass (the tensor
+    cores read it when station x pol is a multiple of 16)."""
     return CorrelateBlock(iring, nframe_per_integration, *args, **kwargs)

@@ -28,6 +28,17 @@
 //    below the diagonal are launched; diagonal tiles load one operand.
 //  * corr_simt_kernel -- shared-memory tiled SIMT fallback for layouts TMA
 //    cannot describe (strides not multiples of 16 B, a.a^H form, ci16/cf32).
+//  * corr4_tc_kernel -- corr_tc_kernel for ci4 input.  TMA moves one byte
+//    per complex sample; the consumers expand the nibbles into the same
+//    K-major int8 layout (tc_transpose_ci4), so everything after the
+//    transpose is shared.
+//
+// ci4 input (extension) enters through bfLinAlgCorrelateCi4 and
+// bfLinAlgCorrelateCi4ToStorage, the ci4 counterparts of the correlator forms
+// of bfLinAlgMatMul and of bfLinAlgCorrelateToStorage.  Those two keep
+// returning BF_STATUS_UNSUPPORTED_DTYPE for ci4, as the reference's
+// bfLinAlgMatMul does, so a caller written against the reference sees its
+// statuses unchanged.
 //
 // bfLinAlgCorrelateToStorage (extension) writes the b^H.b correlation straight
 // in the [baseline][chan][stokes] storage layout of bfVisibilitiesToStorage:
@@ -58,6 +69,20 @@ struct SimtParams {
 
 template<typename I> struct CIn { I x, y; };
 
+// One complex input as float2: I is the component type, or Ci4 for ci4 (one
+// byte, high nibble real, both nibbles two's complement).
+struct Ci4 {};
+template<typename I>
+__device__ __forceinline__ float2 simt_load(const char* p) {
+	CIn<I> v = *(const CIn<I>*)p;
+	return make_float2((float)v.x, (float)v.y);
+}
+template<>
+__device__ __forceinline__ float2 simt_load<Ci4>(const char* p) {
+	const signed char v = *(const signed char*)p;
+	return make_float2((float)(v >> 4), (float)((signed char)(v << 4) >> 4));
+}
+
 template<typename I, typename Acc>
 __global__ void __launch_bounds__(256)
 corr_simt_kernel(SimtParams P) {
@@ -84,14 +109,8 @@ corr_simt_kernel(SimtParams P) {
 			float2 vi = make_float2(0.f, 0.f), vj = make_float2(0.f, 0.f);
 			if( t < P.ntime ) {
 				int gi = ti * 32 + ii, gj = tj * 32 + ii;
-				if( gi < P.n ) {
-					CIn<I> v = *(const CIn<I>*)(ub + (long)t * P.stride_t + (long)gi * P.stride_i);
-					vi = make_float2((float)v.x, (float)v.y);
-				}
-				if( gj < P.n ) {
-					CIn<I> v = *(const CIn<I>*)(ub + (long)t * P.stride_t + (long)gj * P.stride_i);
-					vj = make_float2((float)v.x, (float)v.y);
-				}
+				if( gi < P.n ) vi = simt_load<I>(ub + (long)t * P.stride_t + (long)gi * P.stride_i);
+				if( gj < P.n ) vj = simt_load<I>(ub + (long)t * P.stride_t + (long)gj * P.stride_i);
 			}
 			su_i[tt][ii] = vi; su_j[tt][ii] = vj;
 		}
@@ -153,6 +172,12 @@ enum { TC_KT = 64, TC_STAGES = 3, TC_TILE_BYTES = TC_KT * 128, TC_CONSUMERS = 25
 // split along time (correlate()).
 constexpr long TC_MAX_SUM_LEN   = ((1L << 31) - 1) / (128L * 128L);
 constexpr long PAIR_MAX_SUM_LEN = ((1L << 31) - 1) / (2L * 128L * 128L);
+// ci4 values have |x| <= 8: one Gram entry is bounded by L·8², exact in int32
+// for L <= 33554431, and a pair sum by L·2·8², exact for L <= CI4_MAX_SUM_LEN =
+// 16777215 (2^24 - 1).  Up to that length both ci4 kernels (corr4_tc_kernel,
+// corr_simt_kernel<Ci4, int>) combine in int32 and round to fp32 once, so
+// there is no WIDE variant; correlate() chunks longer ci4 integrations.
+constexpr long CI4_MAX_SUM_LEN  = ((1L << 31) - 1) / (2L * 8L * 8L);
 
 struct TcParams {
 	float2* c; long c_row, c_batch;      // float2 units
@@ -231,6 +256,48 @@ __device__ __forceinline__ void tc_transpose(const unsigned char* raw, unsigned 
 	}
 }
 
+// ci4 counterpart of tc_transpose: the raw TMA tile is raw[k][b] (64 x 64
+// bytes, one byte per complex sample), and kt is what tc_transpose makes of
+// the int8 matrix with row 2b = the high nibble (real) and row 2b + 1 = the
+// low nibble (imaginary), sign-extended.  Each consumer thread expands four
+// 32-bit loads (8 rows x 4 samples) into two 4x4 byte blocks; lanes with odd
+// r8 store their second block first, which keeps the stores at 4-way bank
+// conflicts, as the loads are.
+__device__ __forceinline__ void tc_transpose_ci4(const unsigned char* raw, unsigned char* kt, int tid) {
+	const int l = tid & 31, wq = tid >> 5;
+	const int t4 = (l & 3) | ((wq & 3) << 2);
+	const int r8 = ((l >> 2) & 7) | ((wq >> 2) << 3);
+	const int kf = r8 & 1;                               // the 4-row block stored first
+	const uint32_t sel_f = kf ? 0x7362 : 0x5140, sel_s = kf ? 0x5140 : 0x7362;
+	const uint32_t* src = (const uint32_t*)raw;
+	uint32_t e[2][4];
+#pragma unroll
+	for( int q=0; q<4; ++q ) {
+		const uint32_t w = src[(4 * t4 + q) * 16 + r8];
+		// four nibbles v at once: ((v ^ 8) + 0x78) ^ 0x80 is v sign-extended to
+		// a byte, and no byte carries into the next
+		const uint32_t hi = (((w >> 4) & 0x0F0F0F0Fu) ^ 0x08080808u) + 0x78787878u;
+		const uint32_t lo = ((w & 0x0F0F0F0Fu) ^ 0x08080808u) + 0x78787878u;
+		// rows 8 r8 .. +3 (bytes 0, 1 of w) by 0x5140, rows 8 r8 + 4 .. +7 by 0x7362
+		e[0][q] = __byte_perm(hi, lo, sel_f) ^ 0x80808080u;
+		e[1][q] = __byte_perm(hi, lo, sel_s) ^ 0x80808080u;
+	}
+#pragma unroll
+	for( int k=0; k<2; ++k ) {
+		const int r4 = 2 * r8 + (k ^ kf);
+		const uint32_t a = __byte_perm(e[k][0], e[k][1], 0x5140), b = __byte_perm(e[k][0], e[k][1], 0x7362);
+		const uint32_t c = __byte_perm(e[k][2], e[k][3], 0x5140), d = __byte_perm(e[k][2], e[k][3], 0x7362);
+		const uint32_t o[4] = { __byte_perm(a, c, 0x5410), __byte_perm(a, c, 0x7632),
+		                        __byte_perm(b, d, 0x5410), __byte_perm(b, d, 0x7632) };
+		const int t = 4 * t4;
+#pragma unroll
+		for( int j=0; j<4; ++j ) {
+			const int r = 4 * r4 + j;
+			*(uint32_t*)(kt + ((r >> 3) * 4 + (t >> 4)) * 128 + (r & 7) * 16 + (t & 15)) = o[j];
+		}
+	}
+}
+
 // d = A(64 x 32) . B(32 x 128) + (accumulate ? d : 0), both operands from shared memory
 __device__ __forceinline__ void wgmma_m64n128k32_s8(int (&d)[64], uint64_t da, uint64_t db, int accumulate) {
 	asm volatile(
@@ -266,6 +333,10 @@ __host__ __device__ constexpr size_t tc_smem_bytes() {
 // alias = 1 / 2: A is the same block as B0 / B1 and is not loaded.  Returns in
 // acc[h] the warpgroup's 64 x 128 int32 fragment of column block h (consumer
 // threads only; the producer warp returns false).
+// CI4: the operands are ci4, one byte per complex sample; a [64 k][64 B] box
+// holds the 128 rows of a block (x coordinates in bytes: 64 per block) and
+// fills the first half of its raw tile, which tc_transpose_ci4 expands.
+template<bool CI4 = false>
 __device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtensorMap* ta, const CUtensorMap* tb,
                                             int ax, int az, int bx0, int bz, int nb, int alias, int nk,
                                             int (&acc)[2][64]) {
@@ -285,7 +356,7 @@ __device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtens
 	if( tid >= TC_CONSUMERS ) {
 		// ===================== TMA producer =====================
 		if( tid == TC_CONSUMERS ) {
-			const uint32_t bytes = (uint32_t)TC_TILE_BYTES * (nb + (alias ? 0 : 1));
+			const uint32_t bytes = (uint32_t)(CI4 ? TC_TILE_BYTES / 2 : TC_TILE_BYTES) * (nb + (alias ? 0 : 1));
 			for( int it=0; it<nk; ++it ) {
 				const int s = it % TC_STAGES;
 				const uint32_t ph = (it / TC_STAGES) & 1;
@@ -294,7 +365,7 @@ __device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtens
 				mbar_expect_tx(&full_bar[s], bytes);
 				if( !alias ) tma_load_3d(a, ta, &full_bar[s], ax, it * TC_KT, az);
 				tma_load_3d(a + TC_TILE_BYTES, tb, &full_bar[s], bx0, it * TC_KT, bz);
-				if( nb == 2 ) tma_load_3d(a + 2 * TC_TILE_BYTES, tb, &full_bar[s], bx0 + 128, it * TC_KT, bz);
+				if( nb == 2 ) tma_load_3d(a + 2 * TC_TILE_BYTES, tb, &full_bar[s], bx0 + (CI4 ? 64 : 128), it * TC_KT, bz);
 			}
 		}
 		return false;
@@ -308,9 +379,15 @@ __device__ __forceinline__ bool tc_mainloop(unsigned char* tc_smem, const CUtens
 		mbar_wait(&full_bar[s], ph);
 		const unsigned char* raw = tiles + (size_t)s * TC_STAGE_BYTES;
 		unsigned char* kt = ktbuf + (size_t)(it & 1) * TC_STAGE_BYTES;
-		if( !alias ) tc_transpose(raw, kt, tid);
-		tc_transpose(raw + TC_TILE_BYTES, kt + TC_TILE_BYTES, tid);
-		if( nb == 2 ) tc_transpose(raw + 2 * TC_TILE_BYTES, kt + 2 * TC_TILE_BYTES, tid);
+		if( CI4 ) {
+			if( !alias ) tc_transpose_ci4(raw, kt, tid);
+			tc_transpose_ci4(raw + TC_TILE_BYTES, kt + TC_TILE_BYTES, tid);
+			if( nb == 2 ) tc_transpose_ci4(raw + 2 * TC_TILE_BYTES, kt + 2 * TC_TILE_BYTES, tid);
+		} else {
+			if( !alias ) tc_transpose(raw, kt, tid);
+			tc_transpose(raw + TC_TILE_BYTES, kt + TC_TILE_BYTES, tid);
+			if( nb == 2 ) tc_transpose(raw + 2 * TC_TILE_BYTES, kt + 2 * TC_TILE_BYTES, tid);
+		}
 		// the K-major writes are read by the async proxy (wgmma)
 		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 		mbar_arrive(&empty_bar[s]);
@@ -370,10 +447,10 @@ __device__ __forceinline__ void tc_stage(int const (&acc)[64], float2* staging, 
 		}
 }
 
-template<bool WIDE>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
-	extern __shared__ __align__(1024) unsigned char tc_smem[];
+// corr_tc_kernel<WIDE> (ci8) and corr4_tc_kernel (ci4, x in bytes: 64 per block)
+template<bool WIDE, bool CI4>
+__device__ __forceinline__ void corr_tc_body(unsigned char* tc_smem, const CUtensorMap* tmap, TcParams const& P) {
+	const int bw = CI4 ? 64 : 128;
 	const int batch = blockIdx.y;
 	// Work unit: row block I (128 rows of the real Gram matrix) x a pair of
 	// column blocks (2 JJ, 2 JJ + 1) with 2 JJ <= I.  The second block is
@@ -387,7 +464,7 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 	const int alias = (J0 == I) ? 1 : (nb == 2 && J0 + 1 == I) ? 2 : 0;
 	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
 	int acc[2][64];
-	if( !tc_mainloop(tc_smem, &tmap, &tmap, 128 * I, batch, 128 * J0, batch, nb, alias, nk, acc) ) return;
+	if( !tc_mainloop<CI4>(tc_smem, tmap, tmap, bw * I, batch, bw * J0, batch, nb, alias, nk, acc) ) return;
 
 	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
 	float2* staging = (float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
@@ -417,6 +494,19 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
 	}
 }
 
+template<bool WIDE>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	corr_tc_body<WIDE, false>(tc_smem, &tmap, P);
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr4_tc_kernel(const __grid_constant__ CUtensorMap tmap, TcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	corr_tc_body<false, true>(tc_smem, &tmap, P);
+}
+
 // corr_tc_kernel (alpha 1, beta 0) followed by vis_to_storage_kernel, in one
 // pass: vis[b][chan][stokes] for baselines b = i (i + 1) / 2 + j, i >= j.
 // The 64 x 64 complex tile a column block leaves in staging is 32 stations i
@@ -430,13 +520,14 @@ struct StorageTcParams {
 	int   conj_u;
 };
 
-template<bool WIDE>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-corr_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams P) {
-	extern __shared__ __align__(1024) unsigned char tc_smem[];
+// corr_storage_tc_kernel<WIDE> (ci8) and corr4_storage_tc_kernel (ci4)
+template<bool WIDE, bool CI4>
+__device__ __forceinline__ void corr_storage_tc_body(unsigned char* tc_smem, const CUtensorMap* tmap,
+                                                     StorageTcParams const& P) {
 	// Tiles fastest, as corr_tc_kernel: the CTAs resident together share a
 	// channel's voltages in L2.  Channel fastest (neighbouring 32 B pieces of
 	// the same baselines written together) measured 6-9 % slower (DESIGN.md §5).
+	const int bw = CI4 ? 64 : 128;
 	const int batch = blockIdx.y;
 	int I = 0, rem = blockIdx.x;
 	while( rem >= I / 2 + 1 ) { rem -= I / 2 + 1; ++I; }
@@ -445,7 +536,7 @@ corr_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams
 	const int alias = (J0 == I) ? 1 : (nb == 2 && J0 + 1 == I) ? 2 : 0;
 	const int nk = (P.ntime + TC_KT - 1) / TC_KT;
 	int acc[2][64];
-	if( !tc_mainloop(tc_smem, &tmap, &tmap, 128 * I, batch, 128 * J0, batch, nb, alias, nk, acc) ) return;
+	if( !tc_mainloop<CI4>(tc_smem, tmap, tmap, bw * I, batch, bw * J0, batch, nb, alias, nk, acc) ) return;
 
 	unsigned char* tiles = tc_smem + ((1024u - (smem_u32(tc_smem) & 1023u)) & 1023u);
 	const float2* staging = (const float2*)(tiles + (TC_STAGES + 2) * TC_STAGE_BYTES);
@@ -480,6 +571,19 @@ corr_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams
 		}
 		asm volatile("bar.sync 1, 256;" ::: "memory");   // the TC_CONSUMERS threads
 	}
+}
+
+template<bool WIDE>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	corr_storage_tc_body<WIDE, false>(tc_smem, &tmap, P);
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+corr4_storage_tc_kernel(const __grid_constant__ CUtensorMap tmap, StorageTcParams P) {
+	extern __shared__ __align__(1024) unsigned char tc_smem[];
+	corr_storage_tc_body<false, true>(tc_smem, &tmap, P);
 }
 
 // ---------------------------------------------------------------------------
@@ -602,21 +706,31 @@ struct BFlinalg_impl {
 namespace {
 
 // Whether the tensor-core correlator can read u(t, i) (kernel batch kb with
-// batch stride kb_ustr): ci8, interleaved complex bytes along i, 16-byte time
-// and batch strides that TMA can describe.  The base address is checked per
-// call (its alignment to 16 B).
+// batch stride kb_ustr): ci8 (ci4), contiguous complex samples along i (2 B
+// apart; 1 B for ci4), 16-byte time and batch strides that TMA can describe.
+// The base address is checked per call (its alignment to 16 B).
 bool tc_layout_ok(BFdtype utype, long stride_t, long stride_i, long n, long ntime, long kb, long kb_ustr) {
-	return utype == BF_DTYPE_CI8 && stride_i == 2 && stride_t % 16 == 0 &&
+	return ((utype == BF_DTYPE_CI8 && stride_i == 2) || (utype == BF_DTYPE_CI4 && stride_i == 1)) &&
+	       stride_t % 16 == 0 &&
 	       (kb == 1 || (kb_ustr % 16 == 0 && kb_ustr >= 16)) && n >= 16 && ntime >= 1 &&
 	       get_encode_fn() != nullptr && getenv("BFB_LINALG_SIMT") == nullptr;
 }
 
-// TMA map of nt time samples from ut: [kb][nt][2 n] bytes, [64 t][128 B] boxes.
-bool tc_encode_map(CUtensorMap* tmap, const char* ut, long n, long nt, long stride_t, long kb, long kb_ustr) {
-	cuuint64_t gdim[3] = {(cuuint64_t)(2 * n), (cuuint64_t)nt, (cuuint64_t)kb};
+// Samples per tensor-core pass: the length up to which the kernel's int32
+// sums are exact (with the WIDE epilogue for ci8).
+long tc_max_len(BFdtype utype) {
+	return utype == BF_DTYPE_CI4 ? CI4_MAX_SUM_LEN : TC_MAX_SUM_LEN;
+}
+
+// TMA map of nt time samples from ut: [kb][nt][2 n] bytes with [64 t][128 B]
+// boxes, or for ci4 [kb][nt][n] bytes with [64 t][64 B] boxes.
+bool tc_encode_map(CUtensorMap* tmap, BFdtype utype, const char* ut, long n, long nt, long stride_t, long kb,
+                   long kb_ustr) {
+	const bool ci4 = utype == BF_DTYPE_CI4;
+	cuuint64_t gdim[3] = {(cuuint64_t)(ci4 ? n : 2 * n), (cuuint64_t)nt, (cuuint64_t)kb};
 	cuuint64_t gstr[2] = {(cuuint64_t)stride_t, (cuuint64_t)(kb > 1 ? kb_ustr : stride_t * nt)};
 	if( gstr[1] % 16 ) gstr[1] = round_up<cuuint64_t>(gstr[1], 16);
-	cuuint32_t box[3] = {128, TC_KT, 1};
+	cuuint32_t box[3] = {ci4 ? 64u : 128u, TC_KT, 1};
 	cuuint32_t estr[3] = {1, 1, 1};
 	return get_encode_fn()(tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)ut, gdim, gstr,
 	                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
@@ -651,19 +765,20 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 		float2* cb = (float2*)((char*)cdata + coff);
 		bool use_tc = tc_ok && ((uintptr_t)ub % 16 == 0);
 		// Integer sums are exact only up to a bounded length (TC_MAX_SUM_LEN,
-		// PAIR_MAX_SUM_LEN), so a longer integration runs as consecutive
+		// PAIR_MAX_SUM_LEN, CI4_MAX_SUM_LEN), so a longer integration runs as consecutive
 		// time chunks: the first one applies (alpha, beta), the later ones add
 		// onto c with beta = 1.  A chunk base ub + t0·stride_t stays 16-byte
 		// aligned (stride_t % 16 == 0 on the TC path), so the path holds.
 		long t0 = 0;
 		do {
-			const long maxlen = use_tc ? TC_MAX_SUM_LEN : utype == BF_DTYPE_CI8 ? PAIR_MAX_SUM_LEN : ntime;
+			const long maxlen = use_tc ? tc_max_len(utype) : utype == BF_DTYPE_CI8 ? PAIR_MAX_SUM_LEN :
+			                    utype == BF_DTYPE_CI4 ? CI4_MAX_SUM_LEN : ntime;
 			const long nt = std::min(maxlen, ntime - t0);
 			const char* ut = ub + t0 * stride_t;
 			const float beta_t = t0 == 0 ? (float)beta : 1.f;
 			if( use_tc ) {
 				CUtensorMap tmap;
-				if( !tc_encode_map(&tmap, ut, n, nt, stride_t, kb, kb_ustr) ) { use_tc = false; continue; }   // this chunk again, on SIMT
+				if( !tc_encode_map(&tmap, utype, ut, n, nt, stride_t, kb, kb_ustr) ) { use_tc = false; continue; }   // this chunk again, on SIMT
 				TcParams P;
 				P.c = cb; P.c_row = c_row_bytes / 8; P.c_batch = kb_cstr / 8;
 				P.n = (int)n; P.ntime = (int)nt;
@@ -672,7 +787,8 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 				for( int i=0; i<T; ++i ) P.ntile += i / 2 + 1;     // (row block, column-block pair) units
 				P.alpha = (float)alpha; P.beta = beta_t; P.conj_u = conj_u;
 				const size_t smem = tc_smem_bytes();
-				auto kernel = nt > PAIR_MAX_SUM_LEN ? corr_tc_kernel<true> : corr_tc_kernel<false>;
+				auto kernel = utype == BF_DTYPE_CI4 ? corr4_tc_kernel :
+				              nt > PAIR_MAX_SUM_LEN ? corr_tc_kernel<true> : corr_tc_kernel<false>;
 				BFB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
 				                              (int)smem), BF_STATUS_INTERNAL_ERROR);
 				dim3 grid(P.ntile, (unsigned)kb);
@@ -686,6 +802,7 @@ BFstatus correlate(BFdtype utype, const void* udata, long stride_t, long stride_
 				int T = (int)div_up<long>(n, 32);
 				dim3 grid(T * (T + 1) / 2, (unsigned)kb);
 				switch( utype ) {
+				case BF_DTYPE_CI4:  corr_simt_kernel<Ci4, int><<<grid, 256, 0, st>>>(S); break;
 				case BF_DTYPE_CI8:  corr_simt_kernel<int8_t, int><<<grid, 256, 0, st>>>(S); break;
 				case BF_DTYPE_CI16: corr_simt_kernel<int16_t, float><<<grid, 256, 0, st>>>(S); break;
 				case BF_DTYPE_CF32: corr_simt_kernel<float, float><<<grid, 256, 0, st>>>(S); break;
@@ -943,18 +1060,20 @@ BFstatus bfLinAlgDestroy(BFlinalg handle) {
 	return BF_STATUS_SUCCESS;
 }
 
-BFstatus bfLinAlgMatMul(BFlinalg handle, double alpha, BFarray const* a, BFarray const* b,
-                        double beta, BFarray const* c) {
-	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
-	BFB_ASSERT(a || b, BF_STATUS_INVALID_ARGUMENT);
-	BFB_ASSERT(c, BF_STATUS_INVALID_POINTER);
-	BFB_ASSERT(space_on_device(c->space), BF_STATUS_UNSUPPORTED_SPACE);
-	if( a && b ) { BFB_TRY(return matmul_ab(handle, alpha, a, b, beta, c)); }
+} // extern "C"
+
+namespace {
+
+// The a.a^H / b^H.b forms (one of a, b NULL) of bfLinAlgMatMul (ci4 false:
+// ci8 / ci16 / cf32 input) and of bfLinAlgCorrelateCi4 (ci4 true: ci4 input).
+BFstatus correlate_form(BFlinalg handle, double alpha, BFarray const* a, BFarray const* b,
+                        double beta, BFarray const* c, bool ci4) {
 	BFarray const* x = a ? a : b;
 	BFB_ASSERT(space_on_device(x->space), BF_STATUS_UNSUPPORTED_SPACE);
 	BFB_ASSERT(x->ndim == c->ndim && x->ndim >= 2 && x->ndim <= BF_MAX_DIMS, BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(c->dtype == BF_DTYPE_CF32, BF_STATUS_UNSUPPORTED_DTYPE);
-	BFB_ASSERT(x->dtype == BF_DTYPE_CI8 || x->dtype == BF_DTYPE_CI16 || x->dtype == BF_DTYPE_CF32,
+	BFB_ASSERT(ci4 ? x->dtype == BF_DTYPE_CI4
+	               : x->dtype == BF_DTYPE_CI8 || x->dtype == BF_DTYPE_CI16 || x->dtype == BF_DTYPE_CF32,
 	           BF_STATUS_UNSUPPORTED_DTYPE);
 	int nd = x->ndim;
 	// b^H.b: x is [.., t, i];  a.a^H: x is [.., i, t] and u(t,i) = conj(a[i][t])
@@ -979,6 +1098,29 @@ BFstatus bfLinAlgMatMul(BFlinalg handle, double alpha, BFarray const* a, BFarray
 	                         c->data, c->strides[nd-2], alpha, beta, thread_stream()));
 }
 
+} // namespace
+
+extern "C" {
+
+BFstatus bfLinAlgMatMul(BFlinalg handle, double alpha, BFarray const* a, BFarray const* b,
+                        double beta, BFarray const* c) {
+	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(a || b, BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(c, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(space_on_device(c->space), BF_STATUS_UNSUPPORTED_SPACE);
+	if( a && b ) { BFB_TRY(return matmul_ab(handle, alpha, a, b, beta, c)); }
+	return correlate_form(handle, alpha, a, b, beta, c, false);
+}
+
+BFstatus bfLinAlgCorrelateCi4(BFlinalg handle, double alpha, BFarray const* a, BFarray const* b,
+                              double beta, BFarray const* c) {
+	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT((a != nullptr) != (b != nullptr), BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(c, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(space_on_device(c->space), BF_STATUS_UNSUPPORTED_SPACE);
+	return correlate_form(handle, alpha, a, b, beta, c, true);
+}
+
 } // extern "C"
 
 namespace {
@@ -1000,16 +1142,17 @@ bool correlate_storage_tc(BFarray const* x, BFarray const* vis, BFstatus* status
 	const long nchan = x->shape[0], ntime = x->shape[1], n = x->shape[2];
 	const long kb_ustr = x->strides[0], stride_t = x->strides[1];
 	if( !tc_layout_ok(x->dtype, stride_t, x->strides[2], n, ntime, nchan, kb_ustr) ||
-	    ntime > TC_MAX_SUM_LEN || (uintptr_t)x->data % 16 ) return false;
+	    ntime > tc_max_len(x->dtype) || (uintptr_t)x->data % 16 ) return false;
 	CUtensorMap tmap;
-	if( !tc_encode_map(&tmap, (const char*)x->data, n, ntime, stride_t, nchan, kb_ustr) ) return false;
+	if( !tc_encode_map(&tmap, x->dtype, (const char*)x->data, n, ntime, stride_t, nchan, kb_ustr) ) return false;
 	StorageTcParams P;
 	P.vis = (float2*)vis->data; P.s_base = vis->strides[0] / 8; P.s_chan = vis->strides[1] / 8;
 	P.nstand = (int)(n / 2); P.ntime = (int)ntime; P.conj_u = x->conjugated ? 1 : 0;
 	int T = (int)div_up<long>(2 * n, 128), ntile = 0;
 	for( int i=0; i<T; ++i ) ntile += i / 2 + 1;
 	const size_t smem = tc_smem_bytes();
-	auto kernel = ntime > PAIR_MAX_SUM_LEN ? corr_storage_tc_kernel<true> : corr_storage_tc_kernel<false>;
+	auto kernel = x->dtype == BF_DTYPE_CI4 ? corr4_storage_tc_kernel :
+	              ntime > PAIR_MAX_SUM_LEN ? corr_storage_tc_kernel<true> : corr_storage_tc_kernel<false>;
 	*status = BF_STATUS_SUCCESS;
 	if( cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ) {
 		*status = BF_STATUS_INTERNAL_ERROR;
@@ -1022,15 +1165,14 @@ bool correlate_storage_tc(BFarray const* x, BFarray const* vis, BFstatus* status
 	return true;
 }
 
-} // namespace
-
-extern "C" {
-
-BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis) {
+// bfLinAlgCorrelateToStorage (ci4 false: ci8 / ci16 / cf32 input) and
+// bfLinAlgCorrelateCi4ToStorage (ci4 true: ci4 input).
+BFstatus correlate_to_storage(BFlinalg handle, BFarray const* x, BFarray const* vis, bool ci4) {
 	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
 	BFB_ASSERT(x && vis, BF_STATUS_INVALID_POINTER);
 	BFB_ASSERT(space_on_device(x->space) && space_on_device(vis->space), BF_STATUS_UNSUPPORTED_SPACE);
-	BFB_ASSERT(x->dtype == BF_DTYPE_CI8 || x->dtype == BF_DTYPE_CI16 || x->dtype == BF_DTYPE_CF32,
+	BFB_ASSERT(ci4 ? x->dtype == BF_DTYPE_CI4
+	               : x->dtype == BF_DTYPE_CI8 || x->dtype == BF_DTYPE_CI16 || x->dtype == BF_DTYPE_CF32,
 	           BF_STATUS_UNSUPPORTED_DTYPE);
 	BFB_ASSERT(vis->dtype == BF_DTYPE_CF32, BF_STATUS_UNSUPPORTED_DTYPE);
 	BFB_ASSERT(!vis->conjugated, BF_STATUS_UNSUPPORTED);
@@ -1070,13 +1212,25 @@ BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray c
 	c.ndim = 3;
 	c.shape[0] = nchan; c.shape[1] = n; c.shape[2] = n;
 	c.strides[0] = n * n * 8; c.strides[1] = n * 8; c.strides[2] = 8;
-	status = bfLinAlgMatMul(handle, 1.0, nullptr, x, 0.0, &c);
+	status = correlate_form(handle, 1.0, nullptr, x, 0.0, &c, ci4);
 	if( status != BF_STATUS_SUCCESS ) return status;
 	BFarray m = c;                                   // [nchan][nstand][2][nstand][2]
 	m.ndim = 5;
 	const long shape[5] = {nchan, nstand, 2, nstand, 2}, strides[5] = {n * n * 8, 2 * n * 8, n * 8, 16, 8};
 	for( int d=0; d<5; ++d ) { m.shape[d] = shape[d]; m.strides[d] = strides[d]; }
 	return bfVisibilitiesToStorage(&m, vis);
+}
+
+} // namespace
+
+extern "C" {
+
+BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis) {
+	return correlate_to_storage(handle, x, vis, false);
+}
+
+BFstatus bfLinAlgCorrelateCi4ToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis) {
+	return correlate_to_storage(handle, x, vis, true);
 }
 
 } // extern "C"

@@ -340,6 +340,27 @@ BFstatus bfVisibilitiesFromStorage(BFarray const* in, BFarray const* out);
  * calls through a [nchan, n, n] workspace owned by the handle. */
 BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis);
 
+/* Correlate ci4 voltages: one byte per complex sample, high nibble real, both
+ * nibbles two's complement (the convention of bf.DataType, bfFft, bfMap and
+ * the beamformer).  bfLinAlgMatMul's a.a^H / b^H.b forms and
+ * bfLinAlgCorrelateToStorage return BF_STATUS_UNSUPPORTED_DTYPE for ci4, as
+ * the reference's bfLinAlgMatMul does; these two take ci4 and nothing else,
+ * with the same arguments, shapes, strides and status codes.  Each result is
+ * that of the ci8 call on the same complex integers, bit for bit.
+ * CorrelateCi4: exactly one of a, b is NULL (a.a^H or b^H.b).  b^H.b runs on
+ * the tensor cores when the samples of a time step are contiguous (1 B apart),
+ * the time and batch strides are multiples of 16 B, the base is 16-B aligned
+ * and n >= 16; one pass is exact for ntime <= 16777215 (2^24 - 1), longer
+ * integrations run as exact passes of that length added in fp32.  Every other
+ * layout runs a SIMT kernel (exact to the same length per pass).
+ * CorrelateCi4ToStorage: bfLinAlgCorrelateCi4(handle, 1, NULL, x, 0, C)
+ * followed by bfVisibilitiesToStorage(C, vis), bit for bit; one sm_90a
+ * kernel when the tensor cores take x in one pass, the workspace path
+ * otherwise. */
+BFstatus bfLinAlgCorrelateCi4(BFlinalg handle, double alpha, BFarray const* a, BFarray const* b,
+                              double beta, BFarray const* c);
+BFstatus bfLinAlgCorrelateCi4ToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis);
+
 /* Host-only introspection of the FDMT plan bfFdmtInit would build (no device
  * needed).  step < 0: writes the number of steps to *nrow.  Otherwise writes
  * the row count of `step` to *nrow and, if rows != NULL, nrow triples

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -258,6 +258,9 @@ def main():
     if 'correlate_storage' in ops:
         bench_correlate_storage(stream, rng)
 
+    if 'correlate_ci4' in ops:
+        bench_correlate_ci4(stream, rng)
+
 
 def gpu_name():
     """Card name, power limit and max SM clock, read in the same run as the timings."""
@@ -311,6 +314,53 @@ def bench_correlate_storage(stream, rng, nrep=20):
                two_call_hbm_share=round((vin + 2 * low + vout) / 3.35e12 * 1e3 / two_ms, 3),
                speedup_vs_two_calls=round(two_ms / ms, 3), identical=identical)
         del d_x, xv
+
+
+def bench_correlate_ci4(stream, rng, nrep=20):
+    """The correlator on ci4 voltages, BASELINE config 4 (512 chan, 256
+    stations x 2 pols) as the correlate block passes a ring frame: the ci4 call,
+    bfUnpack to ci8 followed by the ci8 call (what a ci4 pipeline ran before),
+    and the ci8 call alone, timed alternately in the same loop.  The ci4 and
+    ci8 outputs are compared bit for bit.  bfUnpack reads the byte-reversed
+    nibble order, so it unpacks a byte-reversed copy of the same samples."""
+    print(json.dumps({'op': 'correlate_ci4.device', 'gpu': gpu_name()}), flush=True)
+    nchan, n = 512, 512
+    la = bf.linalg.LinAlg()
+    d_c4 = bf.empty((nchan, n, n), 'cf32', 'cuda')
+    d_c8 = bf.empty((nchan, n, n), 'cf32', 'cuda')
+    ci4 = bf.DataType('ci4').as_numpy_dtype()
+    for ntime in (512, 2048, 8192):
+        x4 = rng.integers(0, 256, size=(ntime, nchan, n), dtype=np.uint8).view(ci4)
+        d_x4 = bf.asarray(bf.ndarray(x4, dtype='ci4'), space='cuda')
+        d_x4r = bf.asarray(bf.ndarray(x4, dtype='ci4').byteswap(), space='cuda')
+        del x4
+        d_x8 = bf.empty((ntime, nchan, n), 'ci8', 'cuda')
+        x4v, x8v = d_x4.transpose(1, 0, 2), d_x8.transpose(1, 0, 2)
+        fns = {'ci4': lambda: la.matmul(1, None, x4v, 0, d_c4),
+               'unpack_ci8': lambda: (bf.unpack(d_x4r, d_x8), la.matmul(1, None, x8v, 0, d_c8)),
+               'ci8': lambda: la.matmul(1, None, x8v, 0, d_c8)}
+        for _ in range(2):
+            for fn in fns.values():
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in fns}
+        for _ in range(nrep):
+            for key, fn in fns.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1))
+        identical = bool(np.array_equal(np.asarray(d_c4.copy('system')).view(np.uint64),
+                                        np.asarray(d_c8.copy('system')).view(np.uint64)))
+        ms = {k: float(np.median(v)) for k, v in times.items()}
+        vin, vout = ntime * nchan * n, 8 * nchan * n * (n + 1) // 2
+        report('correlate ci4 ntime=%d n=%d nchan=%d' % (ntime, n, nchan), ms['ci4'], vin + vout,
+               unpack_ci8_ms=round(ms['unpack_ci8'], 4), ci8_ms=round(ms['ci8'], 4),
+               speedup_vs_unpack_ci8=round(ms['unpack_ci8'] / ms['ci4'], 3),
+               vs_ci8_alone=round(ms['ci8'] / ms['ci4'], 3), identical=identical)
+        del d_x4, d_x4r, d_x8, x4v, x8v
 
 
 def bench_beamform(stream, ref, rng):
