@@ -626,28 +626,11 @@ __device__ __forceinline__ void pk_stage_finish(const PackedSmem& S, const Packe
 // i = LS*l .. LS*l + LS-1 in f[]) belongs at row[t0 + i - d] for d <= t0 + i <
 // ntime.  The row's start has whatever alignment d, t0 and the caller's pitch
 // give it, so the lanes regroup their samples on the 16-byte lines of the
-// OUTPUT (three values come from the next lane by shuffle) and write float4s;
-// what is left at the ends of the tile / gulp goes out as scalars.
-template<int LS, int E>
-__device__ __forceinline__ void pk_diag_groups(const float (&x)[LS + 3], float* g, int ibase, int lo, int hi, int lane) {
-#pragma unroll
-	for( int q=0; q<LS/4; ++q ) {
-		const int i0 = ibase + E + 4 * q;
-		const float v0 = x[E + 4*q], v1 = x[E + 4*q + 1], v2 = x[E + 4*q + 2], v3 = x[E + 4*q + 3];
-		if( i0 >= lo && i0 + 4 <= hi ) __stcs((float4*)(g + i0), make_float4(v0, v1, v2, v3));
-		else if( i0 + 4 > lo && i0 < hi ) {
-			if( i0     >= lo && i0     < hi ) __stcs(g + i0,     v0);
-			if( i0 + 1 >= lo && i0 + 1 < hi ) __stcs(g + i0 + 1, v1);
-			if( i0 + 2 >= lo && i0 + 2 < hi ) __stcs(g + i0 + 2, v2);
-			if( i0 + 3 >= lo && i0 + 3 < hi ) __stcs(g + i0 + 3, v3);
-		}
-	}
-	if( E > 0 && lane == 0 ) {
-		// the tile's first E samples precede the first full line
-#pragma unroll
-		for( int j=0; j<E; ++j ) if( j >= lo && j < hi ) __stcs(g + j, x[j]);
-	}
-}
+// OUTPUT: lane l writes i = LS*l + e + 4q .. +3, e the first i on a line
+// (three values come from the next lane by shuffle), and write float4s; what
+// is left at the ends of the tile / gulp goes out as scalars.  The samples are
+// rotated by e with selects, not by a switch over four copies of the stores,
+// so only one set of LS values is live (the switch made ptxas spill).
 template<int LS>
 __device__ __forceinline__ void pk_store_diag(const float (&f)[LS], long d, const PackedParams& P, const PackedTile& tl, int lane) {
 	float* row = (float*)P.dst + tl.doff + d * P.dstride;
@@ -657,17 +640,33 @@ __device__ __forceinline__ void pk_store_diag(const float (&f)[LS], long d, cons
 	const long lo_l = d - tl.t0, hi_l = P.ntime - tl.t0;
 	const int lo = lo_l > 0 ? (int)min(lo_l, (long)P.T) : 0;
 	const int hi = hi_l < (long)P.T ? (int)max(hi_l, 0L) : P.T;
-	float x[LS + 3];
+	float nx[3];
 #pragma unroll
-	for( int k=0; k<LS; ++k ) x[k] = f[k];
+	for( int k=0; k<3; ++k ) nx[k] = __shfl_down_sync(0xffffffffu, f[k], 1);
+	if( e > 0 && lane == 0 ) {
+		// the tile's first e samples precede the first full line
 #pragma unroll
-	for( int k=0; k<3; ++k ) x[LS + k] = __shfl_down_sync(0xffffffffu, f[k], 1);
-	const int ibase = LS * lane;
-	switch( e ) {
-	case 0:  pk_diag_groups<LS, 0>(x, g, ibase, lo, hi, lane); break;
-	case 1:  pk_diag_groups<LS, 1>(x, g, ibase, lo, hi, lane); break;
-	case 2:  pk_diag_groups<LS, 2>(x, g, ibase, lo, hi, lane); break;
-	default: pk_diag_groups<LS, 3>(x, g, ibase, lo, hi, lane); break;
+		for( int j=0; j<3; ++j ) if( j < e && j >= lo && j < hi ) __stcs(g + j, f[j]);
+	}
+	const int ibase = LS * lane + e;
+#pragma unroll
+	for( int q=0; q<LS/4; ++q ) {
+		float v[4];
+#pragma unroll
+		for( int j=0; j<4; ++j ) {
+			const int k = 4 * q + j;                        // v[j] = sample k + e of the lane
+			const float x0 = f[k];
+			const float x1 = k + 1 < LS ? f[k + 1] : nx[k + 1 - LS];
+			const float x2 = k + 2 < LS ? f[k + 2] : nx[k + 2 - LS];
+			const float x3 = k + 3 < LS ? f[k + 3] : nx[k + 3 - LS];
+			v[j] = e == 0 ? x0 : e == 1 ? x1 : e == 2 ? x2 : x3;
+		}
+		const int i0 = ibase + 4 * q;
+		if( i0 >= lo && i0 + 4 <= hi ) __stcs((float4*)(g + i0), make_float4(v[0], v[1], v[2], v[3]));
+		else if( i0 + 4 > lo && i0 < hi ) {
+#pragma unroll
+			for( int j=0; j<4; ++j ) if( i0 + j >= lo && i0 + j < hi ) __stcs(g + i0 + j, v[j]);
+		}
 	}
 }
 
