@@ -7,6 +7,32 @@ from bifrost_b200.blocks import _header as H
 _COMPLEX_IN = ('cf32', 'ci8', 'ci16')
 
 
+def reduce_header(ihdr, axis, factor=None, op='sum'):
+    """(ohdr, axis index, factor, frame factor) of reduce(axis, factor, op) on a
+    sequence with header ihdr; also the header of beamform(..., nint=factor)."""
+    ohdr, otensor = H.derive(ihdr)
+    # power ops give real output; plain ops keep complex input complex
+    keeps_complex = ihdr['_tensor']['dtype'] in _COMPLEX_IN and not op.startswith('pwr')
+    otensor['dtype'] = 'cf32' if keeps_complex else 'f32'
+    axis = H.axis_index(otensor, axis)
+    frame_factor = 1
+    if axis == H.frame_axis(otensor):
+        # along time: fewer frames come out, the shape entry stays -1
+        if factor is None:
+            raise ValueError("Cannot reduce all of the frame axis")
+        frame_factor = factor
+        ohdr['gulp_nframe'] = max((ihdr.get('gulp_nframe') or factor) // factor, 1)
+    else:
+        length = otensor['shape'][axis]
+        if factor is None:
+            factor = length
+        if length % factor:
+            raise ValueError("Reduce factor does not divide axis length")
+        otensor['shape'][axis] = length // factor
+    H.scale_step(otensor, axis, factor)
+    return ohdr, axis, factor, frame_factor
+
+
 class ReduceBlock(TransformBlock):
     def __init__(self, iring, axis, factor=None, op='sum', *args, **kwargs):
         super(ReduceBlock, self).__init__(iring, *args, **kwargs)
@@ -21,27 +47,8 @@ class ReduceBlock(TransformBlock):
         return input_nframe // self.frame_factor
 
     def on_sequence(self, iseq):
-        ihdr = iseq.header
-        ohdr, otensor = H.derive(ihdr)
-        # power ops give real output; plain ops keep complex input complex
-        keeps_complex = ihdr['_tensor']['dtype'] in _COMPLEX_IN and not self.op.startswith('pwr')
-        otensor['dtype'] = 'cf32' if keeps_complex else 'f32'
-        self.axis = H.axis_index(otensor, self.specified_axis)
-        self.factor, self.frame_factor = self.specified_factor, 1
-        if self.axis == H.frame_axis(otensor):
-            # along time: fewer frames come out, the shape entry stays -1
-            if self.factor is None:
-                raise ValueError("Cannot reduce all of the frame axis")
-            self.frame_factor = self.factor
-            ohdr['gulp_nframe'] = max((ihdr.get('gulp_nframe') or self.factor) // self.factor, 1)
-        else:
-            length = otensor['shape'][self.axis]
-            if self.factor is None:
-                self.factor = length
-            if length % self.factor:
-                raise ValueError("Reduce factor does not divide axis length")
-            otensor['shape'][self.axis] = length // self.factor
-        H.scale_step(otensor, self.axis, self.factor)
+        ohdr, self.axis, self.factor, self.frame_factor = reduce_header(
+            iseq.header, self.specified_axis, self.specified_factor, self.op)
         return ohdr
 
     def on_data(self, ispan, ospan):

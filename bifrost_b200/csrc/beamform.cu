@@ -28,6 +28,7 @@
 // Beam tiles of one time tile are adjacent in launch order, so when nbeam >
 // BT the voltages come from HBM once and from L2 for the other beam tiles.
 #include "beamform.hpp"
+#include "detect.cuh"
 
 #include <cstdint>
 
@@ -100,41 +101,33 @@ template<> __device__ __forceinline__ float2 load_weight<W_ci16>(const char* p) 
 }
 
 // Slot `slot` of a voltage chunk: 16 bytes at byte kb0 + 16 (slot % 4) of time
-// sample t0 + slot / 4.  Returns the aligned block that holds its first byte,
-// the byte phase in that block and the number of bytes that belong to the row
-// (0: none, nothing is read).
-__device__ __forceinline__ const uint4* volt_slot(const char* xb, BeamParams const& P, int t0, int slot,
+// sample t0 + slot / 4 (rows at or past tend are empty).  Returns the aligned
+// block that holds its first byte, the byte phase in that block and the number
+// of bytes that belong to the row (0: none, nothing is read).
+__device__ __forceinline__ const uint4* volt_slot(const char* xb, BeamParams const& P, int t0, int tend, int slot,
                                                   long kb0, long row_bytes, int& nval, uint32_t& ph) {
 	const int row = slot >> 2, q = slot & 3;
 	const long off = kb0 + 16 * q;
 	nval = 0; ph = 0;
-	if( t0 + row >= P.ntime || off >= row_bytes ) return nullptr;
+	if( t0 + row >= tend || off >= row_bytes ) return nullptr;
 	const uintptr_t g = (uintptr_t)(xb + (long)(t0 + row) * P.x_time + off);
 	ph = (uint32_t)(g & 15);
 	nval = (int)min(16L, row_bytes - off);
 	return (const uint4*)(g - ph);
 }
 
+// The K loop: re/im[b] = sum_k w[b0 + b][k] x[t0 + tid][k] for the tile's BT
+// beams and the CTA's time samples t0 .. tend-1 (tend - t0 <= BF_NT; threads
+// past tend, and beams past nbeam, sum zeros).  vs and ws are the CTA's
+// staging buffers; the loop ends with a barrier, after which they are free.
 template<typename V, typename W, int BT>
-__global__ void __launch_bounds__(BF_NT, BT <= 2 ? 3 : 2)
-beamform_kernel(BeamParams P) {
+__device__ __forceinline__ void beam_sums(BeamParams const& P, const char* wb, const char* xb, int t0, int tend,
+                                          int b0, unsigned char* vs, float2* ws, float (&re)[BT], float (&im)[BT]) {
 	enum { VS = VoltTraits<V>::SIZE, PW = VoltTraits<V>::PER_WORD, KC = BF_CHUNK / VS };
-	__shared__ __align__(16) unsigned char vs[BF_NT * BF_ROW_PITCH];
-	__shared__ __align__(16) float2 ws[KC * BT];
 	const int tid = threadIdx.x;
-	const int tt = blockIdx.x / P.nbt, bt = blockIdx.x % P.nbt;
-	const int t0 = tt * BF_NT, b0 = bt * BT;
-	long bidx = blockIdx.z, woff = 0, xoff = 0, coff = 0;
-	for( int d=P.nb-1; d>=0; --d ) {
-		const long r = bidx % P.bshape[d]; bidx /= P.bshape[d];
-		woff += r * P.w_b[d]; xoff += r * P.x_b[d]; coff += r * P.c_b[d];
-	}
-	const char* wb = P.w + woff;
-	const char* xb = P.x + xoff;
 	const long row_bytes = (long)P.K * VS;
 	const float xsign = P.conj_x ? -1.f : 1.f, wsign = P.conj_w ? -1.f : 1.f;
 
-	float re[BT], im[BT];
 #pragma unroll
 	for( int b=0; b<BT; ++b ) { re[b] = 0.f; im[b] = 0.f; }
 
@@ -145,7 +138,7 @@ beamform_kernel(BeamParams P) {
 		for( int i=0; i<4; ++i ) {
 			lo[i] = hi[i] = make_uint4(0, 0, 0, 0);
 			int nval; uint32_t ph;
-			const uint4* a = volt_slot(xb, P, t0, tid + BF_NT * i, kb0, row_bytes, nval, ph);
+			const uint4* a = volt_slot(xb, P, t0, tend, tid + BF_NT * i, kb0, row_bytes, nval, ph);
 			if( nval > 0 ) {
 				lo[i] = __ldg(a);
 				if( (int)ph + nval > 16 ) hi[i] = __ldg(a + 1);
@@ -167,7 +160,7 @@ beamform_kernel(BeamParams P) {
 		for( int i=0; i<4; ++i ) {
 			const int slot = tid + BF_NT * i, row = slot >> 2, q = slot & 3;
 			int nval; uint32_t ph;
-			volt_slot(xb, P, t0, slot, kb0, row_bytes, nval, ph);
+			volt_slot(xb, P, t0, tend, slot, kb0, row_bytes, nval, ph);
 			uint4 v = bf_realign(lo[i], hi[i], ph);
 			if( nval < 16 ) {                    // the tail of the row (or no row): zero the rest
 				uint32_t* vw = (uint32_t*)&v;
@@ -214,6 +207,24 @@ beamform_kernel(BeamParams P) {
 		}
 		__syncthreads();
 	}
+}
+
+template<typename V, typename W, int BT>
+__global__ void __launch_bounds__(BF_NT, BT <= 2 ? 3 : 2)
+beamform_kernel(BeamParams P) {
+	enum { VS = VoltTraits<V>::SIZE, KC = BF_CHUNK / VS };
+	__shared__ __align__(16) unsigned char vs[BF_NT * BF_ROW_PITCH];
+	__shared__ __align__(16) float2 ws[KC * BT];
+	const int tid = threadIdx.x;
+	const int tt = blockIdx.x / P.nbt, bt = blockIdx.x % P.nbt;
+	const int t0 = tt * BF_NT, b0 = bt * BT;
+	long bidx = blockIdx.z, woff = 0, xoff = 0, coff = 0;
+	for( int d=P.nb-1; d>=0; --d ) {
+		const long r = bidx % P.bshape[d]; bidx /= P.bshape[d];
+		woff += r * P.w_b[d]; xoff += r * P.x_b[d]; coff += r * P.c_b[d];
+	}
+	float re[BT], im[BT];
+	beam_sums<V, W, BT>(P, P.w + woff, P.x + xoff, t0, P.ntime, b0, vs, ws, re, im);
 
 	// ---- epilogue.  Time-contiguous C: a warp writes 32 consecutive samples
 	// per beam.  Beam-contiguous C: each thread writes its samples' BT beams,
@@ -240,6 +251,107 @@ beamform_kernel(BeamParams P) {
 	}
 }
 
+// ---- power beams: beamform -> detect -> sum over nint samples, in one pass.
+// Each CTA owns a run of whole integration groups (gpc = 256 / nint of them,
+// or one group walked in 256-sample tiles when nint > 256) of one beam tile.
+// Per tile the K loop above runs unchanged, each thread detects its sample's
+// beams from registers (detect.cuh: the arithmetic of bfDetect) into
+// stage[product][sample], and one thread per (group, product) sums the
+// group's samples left to right starting from the first, as bfReduce does;
+// with nint > 256 the sum carries over from one tile to the next in the same
+// thread.  Polarised modes pair beams 2j (x) and 2j+1 (y): b0 is a multiple of
+// BT, and BT >= 2 whenever nbeam >= 2, so a tile never splits a pair.
+enum { BP_PITCH = BF_NT + 1 };     // odd: the summing threads of a warp read distinct banks
+
+struct PowerParams {
+	BeamParams B;
+	char* out; long o_beam, o_prod, o_time, o_b[BF_MAX_DIMS];
+	int mode, npb, nprod, nint, gpc, ngroup;
+};
+
+// stage[o * BP_PITCH] = product o of this thread's sample, o = (beam / npb) * nprod + product.
+template<int BT>
+__device__ __forceinline__ void detect_stage(int mode, const float (&re)[BT], const float (&im)[BT], float* stage) {
+	if( mode == DET_SCALAR ) {
+#pragma unroll
+		for( int b=0; b<BT; ++b ) stage[b * BP_PITCH] = mag2f(make_float2(re[b], im[b]));
+		return;
+	}
+#pragma unroll
+	for( int b=0; b+1<BT; b+=2 ) {
+		const float2 x = make_float2(re[b], im[b]), y = make_float2(re[b + 1], im[b + 1]);
+		float o[4];
+		if( mode == DET_STOKES_I ) {
+			detect_pol<DET_STOKES_I>(x, y, o);
+			stage[(b / 2) * BP_PITCH] = o[0];
+			continue;
+		}
+		if( mode == DET_STOKES ) detect_pol<DET_STOKES>(x, y, o);
+		else                     detect_pol<DET_COHERENCE>(x, y, o);
+#pragma unroll
+		for( int q=0; q<4; ++q ) stage[(2 * b + q) * BP_PITCH] = o[q];
+	}
+}
+
+template<typename V, typename W, int BT>
+__global__ void __launch_bounds__(BF_NT, BT <= 2 ? 3 : 2)
+beam_power_kernel(const __grid_constant__ PowerParams Q) {
+	enum { VS = VoltTraits<V>::SIZE, KC = BF_CHUNK / VS,
+	       LOOP_BYTES = BF_NT * BF_ROW_PITCH + KC * BT * 8, STAGE_BYTES = 2 * BT * BP_PITCH * 4 };
+	// the K loop's buffers and the detected products share one allocation
+	__shared__ __align__(16) unsigned char smem[LOOP_BYTES > STAGE_BYTES ? LOOP_BYTES : STAGE_BYTES];
+	unsigned char* vs = smem;
+	float2* ws = (float2*)(smem + BF_NT * BF_ROW_PITCH);
+	float* stage = (float*)smem;
+	BeamParams const& P = Q.B;
+	const int tid = threadIdx.x;
+	const int tt = blockIdx.x / P.nbt, bt = blockIdx.x % P.nbt;
+	const int b0 = bt * BT;
+	long bidx = blockIdx.z, woff = 0, xoff = 0, ooff = 0;
+	for( int d=P.nb-1; d>=0; --d ) {
+		const long r = bidx % P.bshape[d]; bidx /= P.bshape[d];
+		woff += r * P.w_b[d]; xoff += r * P.x_b[d]; ooff += r * Q.o_b[d];
+	}
+	const int nint = Q.nint, nprod = Q.nprod, npb = Q.npb;
+	const int no = BT / npb * nprod;                   // staged products per sample
+	const int g0 = tt * Q.gpc;                          // first integration group
+	const int start = g0 * nint, cend = min(g0 + Q.gpc, Q.ngroup) * nint;
+	const bool whole = nint <= BF_NT;                   // every tile holds whole groups
+	float carry = 0.f;
+	for( int s = start; s < cend; s += BF_NT ) {
+		const int tend = min(s + BF_NT, cend);
+		float re[BT], im[BT];
+		beam_sums<V, W, BT>(P, P.w + woff, P.x + xoff, s, tend, b0, vs, ws, re, im);
+		detect_stage<BT>(Q.mode, re, im, stage + tid);
+		__syncthreads();
+		const int len = whole ? nint : tend - s, ng = whole ? (tend - s) / nint : 1;
+		const bool first = whole || s == start, last = whole || tend == cend;
+		for( int j = tid; j < ng * no; j += BF_NT ) {
+			const int o = j % no, g = j / no;
+			const float* src = stage + o * BP_PITCH + g * len;
+			float a = first ? src[0] : carry;
+			for( int i = first ? 1 : 0; i < len; ++i ) a += src[i];
+			if( !last ) { carry = a; continue; }
+			const int ob = o / nprod, q = o % nprod;
+			if( b0 + ob * npb >= P.nbeam ) continue;
+			*(float*)(Q.out + ooff + (long)(b0 / npb + ob) * Q.o_beam + (long)q * Q.o_prod +
+			          (long)(g0 + g) * Q.o_time) = a;
+		}
+		__syncthreads();
+	}
+}
+
+template<typename V, typename W>
+static void launch_power_bt(int bt, dim3 grid, PowerParams const& Q, cudaStream_t st) {
+	switch( bt ) {
+	case 1:  beam_power_kernel<V, W, 1><<<grid, BF_NT, 0, st>>>(Q); break;
+	case 2:  beam_power_kernel<V, W, 2><<<grid, BF_NT, 0, st>>>(Q); break;
+	case 4:  beam_power_kernel<V, W, 4><<<grid, BF_NT, 0, st>>>(Q); break;
+	case 8:  beam_power_kernel<V, W, 8><<<grid, BF_NT, 0, st>>>(Q); break;
+	default: beam_power_kernel<V, W, 16><<<grid, BF_NT, 0, st>>>(Q); break;
+	}
+}
+
 template<typename V, typename W>
 static void launch_bt(int bt, dim3 grid, BeamParams const& P, cudaStream_t st) {
 	switch( bt ) {
@@ -251,9 +363,7 @@ static void launch_bt(int bt, dim3 grid, BeamParams const& P, cudaStream_t st) {
 	}
 }
 
-BFstatus beamform_launch(BeamformOperands const& op, cudaStream_t st) {
-	BFB_ASSERT(op.nbatch >= 1 && op.nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
-	BeamParams P;
+static void beam_params(BeamformOperands const& op, BeamParams& P) {
 	P.w = (const char*)op.w; P.w_beam = op.w_beam;
 	P.x = (const char*)op.x; P.x_time = op.x_time;
 	P.c = (char*)op.c; P.c_beam = op.c_beam; P.c_time = op.c_time;
@@ -264,8 +374,20 @@ BFstatus beamform_launch(BeamformOperands const& op, cudaStream_t st) {
 	P.nbeam = op.nbeam; P.ntime = op.ntime; P.K = op.K;
 	P.alpha = (float)op.alpha; P.beta = (float)op.beta;
 	P.conj_w = op.conj_w; P.conj_x = op.conj_x;
+}
+
+// Beams per tile: the power of two up to 16 that covers nbeam.
+static int beam_tile(int nbeam) {
 	int bt = 1;
-	while( bt < op.nbeam && bt < 16 ) bt *= 2;
+	while( bt < nbeam && bt < 16 ) bt *= 2;
+	return bt;
+}
+
+BFstatus beamform_launch(BeamformOperands const& op, cudaStream_t st) {
+	BFB_ASSERT(op.nbatch >= 1 && op.nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
+	BeamParams P;
+	beam_params(op, P);
+	const int bt = beam_tile(op.nbeam);
 	P.nbt = (int)div_up<long>(op.nbeam, bt);
 	const long nblk = div_up<long>(op.ntime, BF_NT) * P.nbt;
 	BFB_ASSERT(nblk <= 0x7FFFFFFFL, BF_STATUS_UNSUPPORTED_SHAPE);
@@ -273,6 +395,32 @@ BFstatus beamform_launch(BeamformOperands const& op, cudaStream_t st) {
 	const bool ci4 = op.xtype == BF_DTYPE_CI4, ci16 = op.wtype == BF_DTYPE_CI16;
 	if( ci4 ) { if( ci16 ) launch_bt<V_ci4, W_ci16>(bt, grid, P, st); else launch_bt<V_ci4, W_cf32>(bt, grid, P, st); }
 	else      { if( ci16 ) launch_bt<V_ci8, W_ci16>(bt, grid, P, st); else launch_bt<V_ci8, W_cf32>(bt, grid, P, st); }
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	return BF_STATUS_SUCCESS;
+}
+
+BFstatus beam_power_launch(BeamformOperands const& op, BeamPowerOut const& o, cudaStream_t st) {
+	BFB_ASSERT(op.nbatch >= 1 && op.nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
+	BFB_ASSERT(o.nint >= 1 && op.ntime % o.nint == 0, BF_STATUS_INVALID_SHAPE);
+	PowerParams Q;
+	beam_params(op, Q.B);
+	const int bt = beam_tile(op.nbeam);
+	Q.B.nbt = (int)div_up<long>(op.nbeam, bt);
+	Q.out = (char*)o.out; Q.o_beam = o.o_beam; Q.o_prod = o.o_prod; Q.o_time = o.o_time;
+	for( int d=0; d<op.nb; ++d ) Q.o_b[d] = o.o_b[d];
+	Q.mode = o.mode;
+	Q.npb = o.mode == DET_SCALAR ? 1 : 2;
+	Q.nprod = o.mode == DET_SCALAR ? 1 : detect_nprod(o.mode);
+	Q.nint = o.nint;
+	Q.gpc = o.nint <= BF_NT ? BF_NT / o.nint : 1;
+	Q.ngroup = op.ntime / o.nint;
+	const long nblk = div_up<long>(Q.ngroup, Q.gpc) * Q.B.nbt;
+	BFB_ASSERT(nblk <= 0x7FFFFFFFL, BF_STATUS_UNSUPPORTED_SHAPE);
+	dim3 grid((unsigned)nblk, 1, (unsigned)op.nbatch);
+	const bool ci4 = op.xtype == BF_DTYPE_CI4, ci16 = op.wtype == BF_DTYPE_CI16;
+	if( ci4 ) { if( ci16 ) launch_power_bt<V_ci4, W_ci16>(bt, grid, Q, st); else launch_power_bt<V_ci4, W_cf32>(bt, grid, Q, st); }
+	else      { if( ci16 ) launch_power_bt<V_ci8, W_ci16>(bt, grid, Q, st); else launch_power_bt<V_ci8, W_cf32>(bt, grid, Q, st); }
 	count_launch();
 	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 	return BF_STATUS_SUCCESS;

@@ -19,4 +19,16 @@ struct BeamformOperands {
 
 BFstatus beamform_launch(BeamformOperands const& op, cudaStream_t st);
 
+// Power beams from the same product (op.c, c_* and alpha, beta unused):
+// out[batch][beam / npb][prod][t / nint] = sum over the nint samples of group
+// t / nint of the detected products (detect.cuh) of beams c[.][beam][t], with
+// npb = 1 for mode scalar and 2 (beam pairs 2j, 2j+1 as pol x, y) for stokes,
+// stokes_i and coherence.  f32 out, byte strides; o_b runs over op's batch dims.
+struct BeamPowerOut {
+	void* out; long o_beam, o_prod, o_time, o_b[BF_MAX_DIMS];
+	int mode, nint;
+};
+
+BFstatus beam_power_launch(BeamformOperands const& op, BeamPowerOut const& o, cudaStream_t st);
+
 } // namespace bfb

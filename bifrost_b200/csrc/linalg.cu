@@ -47,6 +47,7 @@
 #include "core.hpp"
 #include "shape.hpp"
 #include "beamform.hpp"
+#include "detect.cuh"
 #include "stokes.cuh"
 
 #include <cuda.h>
@@ -700,7 +701,14 @@ struct BFlinalg_impl {
 	// cf32 [nchan][n][n] matrix of bfLinAlgCorrelateToStorage's workspace path, grown on demand
 	void*  vis_buf = nullptr;
 	size_t vis_size = 0;
-	~BFlinalg_impl() { if( at_buf ) cudaFree(at_buf); if( vis_buf ) cudaFree(vis_buf); }
+	// cf32 beams and f32 detected beams of bfLinAlgBeamformDetect's workspace path, grown on demand
+	void*  pow_buf = nullptr;
+	size_t pow_size = 0;
+	~BFlinalg_impl() {
+		if( at_buf ) cudaFree(at_buf);
+		if( vis_buf ) cudaFree(vis_buf);
+		if( pow_buf ) cudaFree(pow_buf);
+	}
 };
 
 namespace {
@@ -973,29 +981,44 @@ static bool matmul_ab_tc(BFlinalg_impl* h, AbParams const& P, long nbatch, BFsta
 // The beamformer (beamform.cu), when the operands allow it (returns false to
 // leave the call to the other kernels): cf32 / ci16 weights a times ci4 / ci8
 // voltages b into cf32, unit stride along K in both, 8-byte multiple C strides.
-static bool matmul_ab_beamform(AbParams const& P, long nbatch, BFstatus* status) {
+// Whether the beamformer takes the weights a and voltages b of P (C aside),
+// and if so their operands in *op.
+static bool beamform_operands(AbParams const& P, long nbatch, BeamformOperands* op) {
 	if( getenv("BFB_LINALG_SIMT") ) return false;
 	const long wsz = P.a.kind == BF_DTYPE_CF32 ? 8 : P.a.kind == BF_DTYPE_CI16 ? 4 : 0;
 	const long xsz = P.b.kind == BF_DTYPE_CI8 ? 2 : P.b.kind == BF_DTYPE_CI4 ? 1 : 0;
-	if( !wsz || !xsz || P.c_kind != BF_DTYPE_CF32 || P.a.sk != wsz || P.b.sk != xsz || P.K < 1 ) return false;
-	if( P.c_m % 8 || P.c_n % 8 || (uintptr_t)P.c % 8 || (uintptr_t)P.a.p % wsz || P.a.sm % wsz ) return false;
-	BeamformOperands op;
+	if( !wsz || !xsz || P.a.sk != wsz || P.b.sk != xsz || P.K < 1 ) return false;
+	if( (uintptr_t)P.a.p % wsz || P.a.sm % wsz ) return false;
 	for( int d=0; d<P.nb; ++d ) {
-		if( P.c_b[d] % 8 || P.a.sb[d] % wsz ) return false;
-		op.w_b[d] = P.a.sb[d]; op.x_b[d] = P.b.sb[d]; op.c_b[d] = P.c_b[d]; op.bshape[d] = P.bshape[d];
+		if( P.a.sb[d] % wsz ) return false;
+		op->w_b[d] = P.a.sb[d]; op->x_b[d] = P.b.sb[d]; op->bshape[d] = P.bshape[d];
 	}
-	op.wtype = (BFdtype)P.a.kind; op.xtype = (BFdtype)P.b.kind;
-	op.w = P.a.p; op.w_beam = P.a.sm; op.conj_w = P.a.conj;
-	op.x = P.b.p; op.x_time = P.b.sm; op.conj_x = P.b.conj;
+	op->wtype = (BFdtype)P.a.kind; op->xtype = (BFdtype)P.b.kind;
+	op->w = P.a.p; op->w_beam = P.a.sm; op->conj_w = P.a.conj;
+	op->x = P.b.p; op->x_time = P.b.sm; op->conj_x = P.b.conj;
+	op->nb = P.nb; op->nbatch = nbatch;
+	op->nbeam = P.M; op->ntime = P.N; op->K = P.K;
+	return true;
+}
+
+static bool matmul_ab_beamform(AbParams const& P, long nbatch, BFstatus* status) {
+	BeamformOperands op;
+	if( P.c_kind != BF_DTYPE_CF32 || !beamform_operands(P, nbatch, &op) ) return false;
+	if( P.c_m % 8 || P.c_n % 8 || (uintptr_t)P.c % 8 ) return false;
+	for( int d=0; d<P.nb; ++d ) {
+		if( P.c_b[d] % 8 ) return false;
+		op.c_b[d] = P.c_b[d];
+	}
 	op.c = P.c; op.c_beam = P.c_m; op.c_time = P.c_n;
-	op.nb = P.nb; op.nbatch = nbatch;
-	op.nbeam = P.M; op.ntime = P.N; op.K = P.K;
 	op.alpha = P.alpha; op.beta = P.beta;
 	*status = beamform_launch(op, thread_stream());
 	return true;
 }
 
-static BFstatus matmul_ab(BFlinalg_impl* handle, double alpha, BFarray const* a, BFarray const* b, double beta, BFarray const* c) {
+// The operands of c = alpha a.b + beta c, batch dims following c (a and b
+// broadcast where their extent is 1).
+static BFstatus ab_parse(double alpha, BFarray const* a, BFarray const* b, double beta, BFarray const* c,
+                         AbParams* out, long* nbatch_out) {
 	BFB_ASSERT(space_on_device(a->space) && space_on_device(b->space), BF_STATUS_UNSUPPORTED_SPACE);
 	int nd = c->ndim;
 	BFB_ASSERT(a->ndim == nd && b->ndim == nd && nd >= 2 && nd <= BF_MAX_DIMS, BF_STATUS_INVALID_SHAPE);
@@ -1026,8 +1049,18 @@ static BFstatus matmul_ab(BFlinalg_impl* handle, double alpha, BFarray const* a,
 		nbatch *= c->shape[d];
 		++P.nb;
 	}
+	if( P.M != 0 && P.N != 0 && nbatch != 0 ) BFB_ASSERT(nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
+	*out = P;
+	*nbatch_out = nbatch;
+	return BF_STATUS_SUCCESS;
+}
+
+static BFstatus matmul_ab(BFlinalg_impl* handle, double alpha, BFarray const* a, BFarray const* b, double beta, BFarray const* c) {
+	AbParams P;
+	long nbatch;
+	BFstatus st = ab_parse(alpha, a, b, beta, c, &P, &nbatch);
+	if( st != BF_STATUS_SUCCESS ) return st;
 	if( P.M == 0 || P.N == 0 || nbatch == 0 ) return BF_STATUS_SUCCESS;
-	BFB_ASSERT(nbatch <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);
 	{
 		BFstatus tcs = BF_STATUS_SUCCESS;
 		if( matmul_ab_beamform(P, nbatch, &tcs) ) return tcs;
@@ -1231,6 +1264,95 @@ BFstatus bfLinAlgCorrelateToStorage(BFlinalg handle, BFarray const* x, BFarray c
 
 BFstatus bfLinAlgCorrelateCi4ToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis) {
 	return correlate_to_storage(handle, x, vis, true);
+}
+
+} // extern "C"
+
+namespace {
+
+// A contiguous device array descriptor over `data`.
+BFarray dense_array(void* data, BFdtype dtype, int ndim, const long* shape) {
+	BFarray a;
+	std::memset(&a, 0, sizeof(a));
+	a.data = data; a.space = BF_SPACE_CUDA; a.dtype = dtype; a.ndim = ndim;
+	long stride = dtype_nbyte(dtype);
+	for( int d=ndim-1; d>=0; --d ) { a.shape[d] = shape[d]; a.strides[d] = stride; stride *= shape[d]; }
+	return a;
+}
+
+BFstatus beamform_detect(BFlinalg handle, BFarray const* w, BFarray const* x, int mode, int nint,
+                         BFarray const* out) {
+	BFB_ASSERT(handle, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(w && x && out, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(mode == DET_SCALAR || mode == DET_STOKES || mode == DET_STOKES_I || mode == DET_COHERENCE,
+	           BF_STATUS_UNSUPPORTED);
+	BFB_ASSERT(space_on_device(out->space), BF_STATUS_UNSUPPORTED_SPACE);
+	BFB_ASSERT(out->dtype == BF_DTYPE_F32, BF_STATUS_UNSUPPORTED_DTYPE);
+	const int nd = w->ndim;
+	BFB_ASSERT(nint >= 1, BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(nd >= 2 && nd <= BF_MAX_DIMS - 1 && x->ndim == nd && out->ndim == nd + 1, BF_STATUS_INVALID_SHAPE);
+	const long nbeam = w->shape[nd-2], ntime = x->shape[nd-1];
+	const int npb = mode == DET_SCALAR ? 1 : 2, nprod = mode == DET_SCALAR ? 1 : detect_nprod(mode);
+	BFB_ASSERT(ntime % nint == 0 && nbeam % npb == 0, BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(out->shape[nd-2] == nbeam / npb && out->shape[nd-1] == nprod && out->shape[nd] == ntime / nint,
+	           BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT((uintptr_t)out->data % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	for( int d=0; d<=nd; ++d )
+		BFB_ASSERT(out->shape[d] == 1 || (out->strides[d] > 0 && out->strides[d] % 4 == 0), BF_STATUS_UNSUPPORTED_STRIDE);
+	// C = w.x: cf32 [batch.., nbeam, ntime] with out's batch dims
+	long cshape[BF_MAX_DIMS];
+	for( int d=0; d<nd-2; ++d ) cshape[d] = out->shape[d];
+	cshape[nd-2] = nbeam; cshape[nd-1] = ntime;
+	BFarray c = dense_array(nullptr, BF_DTYPE_CF32, nd, cshape);
+	AbParams P;
+	long nbatch;
+	BFstatus status = ab_parse(1.0, w, x, 0.0, &c, &P, &nbatch);
+	if( status != BF_STATUS_SUCCESS ) return status;
+	if( P.M == 0 || P.N == 0 || nbatch == 0 ) return BF_STATUS_SUCCESS;
+	BeamformOperands op;
+	if( beamform_operands(P, nbatch, &op) ) {
+		BeamPowerOut o;
+		o.out = out->data;
+		o.o_beam = out->strides[nd-2]; o.o_prod = out->strides[nd-1]; o.o_time = out->strides[nd];
+		for( int d=0, k=0; d<nd-2; ++d )
+			if( c.shape[d] != 1 ) o.o_b[k++] = out->strides[d];
+		o.mode = mode; o.nint = nint;
+		return beam_power_launch(op, o, thread_stream());
+	}
+	// Workspace path: the three calls of the definition, so the bits hold for every input.
+	long dshape[BF_MAX_DIMS];                         // detected: [batch.., nbeam / npb, nprod, ntime]
+	for( int d=0; d<nd-2; ++d ) dshape[d] = out->shape[d];
+	dshape[nd-2] = nbeam / npb; dshape[nd-1] = nprod; dshape[nd] = ntime;
+	const size_t cbytes = round_up<size_t>((size_t)array_numel(&c) * 8, 256);
+	const size_t need = cbytes + (nint > 1 ? (size_t)array_numel(&c) / npb * nprod * 4 : 0);
+	if( handle->pow_size < need ) {
+		cudaStreamSynchronize(thread_stream());
+		if( handle->pow_buf ) cudaFree(handle->pow_buf);
+		handle->pow_buf = nullptr; handle->pow_size = 0;
+		BFB_ASSERT(cudaMalloc(&handle->pow_buf, need) == cudaSuccess, BF_STATUS_MEM_ALLOC_FAILED);
+		handle->pow_size = need;
+	}
+	c.data = handle->pow_buf;
+	status = matmul_ab(handle, 1.0, w, x, 0.0, &c);
+	if( status != BF_STATUS_SUCCESS ) return status;
+	BFarray cp = c;                                   // [batch.., nbeam / npb, npb, ntime]
+	cp.ndim = nd + 1;
+	cp.shape[nd-2] = nbeam / npb; cp.shape[nd-1] = npb; cp.shape[nd] = ntime;
+	cp.strides[nd-2] = npb * ntime * 8; cp.strides[nd-1] = ntime * 8; cp.strides[nd] = 8;
+	if( nint == 1 ) return bfDetect(&cp, out, mode, nd - 1);
+	BFarray det = dense_array((char*)handle->pow_buf + cbytes, BF_DTYPE_F32, nd + 1, dshape);
+	status = bfDetect(&cp, &det, mode, nd - 1);
+	if( status != BF_STATUS_SUCCESS ) return status;
+	return bfReduce(&det, out, BF_REDUCE_SUM);
+}
+
+} // namespace
+
+extern "C" {
+
+BFstatus bfLinAlgBeamformDetect(BFlinalg handle, BFarray const* w, BFarray const* x, int mode, int nint,
+                                BFarray const* out) {
+	BFB_TRY(return beamform_detect(handle, w, x, mode, nint, out));
 }
 
 } // extern "C"

@@ -10,6 +10,7 @@
 // x*conj(y) = (fma(xi,yi,xr*yr), fma(xr,-yi,xi*yr)) (src/Complex.hpp:194-200).
 // Integer-complex inputs are converted unscaled (src/Complex.hpp:182-184).
 #include "core.hpp"
+#include "detect.cuh"
 #include "shape.hpp"
 
 #include <algorithm>
@@ -25,8 +26,6 @@ BFstatus map_jit(int ndim, long const* shape, char const* const* axis_names, int
                  BFarray const* const* args, char const* const* arg_names, char const* func_name,
                  char const* func, char const* extra_code, int const* block_axes, bool compile_only, int* mode_out);
 void map_jit_clear_cache();
-
-enum DetectMode { DET_SCALAR = 0, DET_JONES = 1, DET_STOKES = 2, DET_STOKES_I = 3, DET_COHERENCE = 4 };
 
 struct EltParams {
 	int  ndim;
@@ -44,7 +43,6 @@ __device__ __forceinline__ float2 load_cplx(const char* p) {
 	CplxOf<I> c = *(const CplxOf<I>*)p;
 	return make_float2((float)c.x, (float)c.y);
 }
-__device__ __forceinline__ float mag2f(float2 z) { float a = z.x * z.x; a += z.y * z.y; return a; }
 
 template<typename I, int MODE>
 __global__ void __launch_bounds__(256)
@@ -68,29 +66,22 @@ detect_kernel(const char* __restrict__ in, char* __restrict__ out, EltParams p) 
 			continue;
 		}
 		float2 y = load_cplx<I>(in + ioff + p.ipol);
-		float xx = mag2f(x), yy = mag2f(y);
-		if( MODE == DET_STOKES_I ) {
-			*(float*)(out + ooff) = xx + yy;
-		} else if( MODE == DET_JONES ) {
+		if( MODE == DET_JONES ) {
 			// b(pol0) = (|x|^2, |y|^2);  b(pol1) = x * conj(y)
+			float xx = mag2f(x), yy = mag2f(y);
 			float re = x.x * y.x;  re -= x.y * (-y.y);
 			float im = x.y * y.x;  im += x.x * (-y.y);
 			*(float2*)(out + ooff)          = make_float2(xx, yy);
 			*(float2*)(out + ooff + p.opol) = make_float2(re, im);
-		} else if( MODE == DET_STOKES ) {
-			float re = x.x * y.x;  re -= x.y * (-y.y);
-			float im = x.y * y.x;  im += x.x * (-y.y);
-			*(float*)(out + ooff)            = xx + yy;
-			*(float*)(out + ooff +   p.opol) = xx - yy;
-			*(float*)(out + ooff + 2*p.opol) =  2 * re;
-			*(float*)(out + ooff + 3*p.opol) = -2 * im;
-		} else {   // coherence: conj(x) * y
-			float re = x.x * y.x;     re -= (-x.y) * y.y;
-			float im = (-x.y) * y.x;  im += x.x * y.y;
-			*(float*)(out + ooff)            = xx;
-			*(float*)(out + ooff +   p.opol) = yy;
-			*(float*)(out + ooff + 2*p.opol) = re;
-			*(float*)(out + ooff + 3*p.opol) = im;
+			continue;
+		}
+		float o[4];
+		detect_pol<MODE>(x, y, o);
+		*(float*)(out + ooff) = o[0];
+		if( MODE != DET_STOKES_I ) {
+			*(float*)(out + ooff +   p.opol) = o[1];
+			*(float*)(out + ooff + 2*p.opol) = o[2];
+			*(float*)(out + ooff + 3*p.opol) = o[3];
 		}
 	}
 }
@@ -129,17 +120,10 @@ detect_vec4_kernel(const char* __restrict__ in, char* __restrict__ out, EltParam
 		                     make_float2(yb.x, yb.y), make_float2(yb.z, yb.w)};
 #pragma unroll
 		for( int k=0; k<4; ++k ) {
-			float xx = mag2f(x[k]), yy = mag2f(y[k]);
-			if( MODE == DET_STOKES_I ) { o0[k] = xx + yy; }
-			else if( MODE == DET_STOKES ) {
-				float re = x[k].x * y[k].x;  re -= x[k].y * (-y[k].y);
-				float im = x[k].y * y[k].x;  im += x[k].x * (-y[k].y);
-				o0[k] = xx + yy; o1[k] = xx - yy; o2[k] = 2 * re; o3[k] = -2 * im;
-			} else {   // coherence: conj(x) * y
-				float re = x[k].x * y[k].x;     re -= (-x[k].y) * y[k].y;
-				float im = (-x[k].y) * y[k].x;  im += x[k].x * y[k].y;
-				o0[k] = xx; o1[k] = yy; o2[k] = re; o3[k] = im;
-			}
+			float o[4];
+			detect_pol<MODE>(x[k], y[k], o);
+			o0[k] = o[0];
+			if( MODE != DET_STOKES_I ) { o1[k] = o[1]; o2[k] = o[2]; o3[k] = o[3]; }
 		}
 		*(float4*)(out + ooff) = make_float4(o0[0], o0[1], o0[2], o0[3]);
 		if( MODE != DET_STOKES_I ) {

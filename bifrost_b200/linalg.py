@@ -1,6 +1,7 @@
 """bf.linalg.LinAlg (mirrors python/bifrost/linalg.py:38-67 -> bfLinAlg*)."""
 from bifrost_b200.libbifrost import _bf, _check, BifrostObject
 from bifrost_b200.ndarray import asarray
+from bifrost_b200.map import DETECT_MODES
 
 
 class LinAlg(BifrostObject):
@@ -35,3 +36,16 @@ class LinAlg(BifrostObject):
             _bf.bfLinAlgCorrelateToStorage
         _check(fn(self.obj, x_array, asarray(vis).as_BFarray()))
         return vis
+
+    def beamform_detect(self, w, x, out, mode='stokes', nint=1):
+        """out = power beams of w.x: the beams C = w.x (w [..., nb, K],
+        x [..., K, ntime], as matmul's a.b), detected with `mode` ('scalar',
+        'stokes', 'stokes_i' or 'coherence'; polarised modes take beam rows
+        2j, 2j+1 as pols x, y of beam j) and summed over nint samples:
+        out f32 [..., nb/npb, nprod, ntime/nint].  Bit for bit
+        reduce(detect(matmul(1, w, x, 0, C) as [..., nb/npb, npb, ntime]), nint),
+        in one kernel for cf32 / ci16 w and ci4 / ci8 x (bfLinAlgBeamformDetect)."""
+        m = DETECT_MODES[mode] if isinstance(mode, str) else int(mode)
+        _check(_bf.bfLinAlgBeamformDetect(self.obj, asarray(w).as_BFarray(), asarray(x).as_BFarray(),
+                                          m, int(nint), asarray(out).as_BFarray()))
+        return out

@@ -167,7 +167,11 @@ class Pipeline(object):
         bfSpectrometerFused) between the chain's input and output rings; and a
         correlate(...) feeding only a convert_visibilities(..., 'storage'), both
         created under fuse=True, by one correlate(..., output='storage')
-        (bfLinAlgCorrelateToStorage: the same output bits, one HBM pass fewer)."""
+        (bfLinAlgCorrelateToStorage: the same output bits, one HBM pass fewer);
+        and a beamform(w) -> detect(mode) -> reduce('time', nint, op='sum'),
+        mode scalar / stokes / stokes_i / coherence, each feeding only the
+        next, by one beamform(w, detect=mode, nint=nint)
+        (bfLinAlgBeamformDetect: the same output bits and header, one kernel)."""
         from bifrost_b200.blocks.transpose import TransposeBlock
         from bifrost_b200.blocks.fft import FftBlock
         from bifrost_b200.blocks.detect import DetectBlock
@@ -176,6 +180,7 @@ class Pipeline(object):
         from bifrost_b200.blocks.spectrometer import SpectrometerBlock
         from bifrost_b200.blocks.correlate import CorrelateBlock
         from bifrost_b200.blocks.convert_visibilities import ConvertVisibilitiesBlock
+        from bifrost_b200.blocks.beamform import BeamformBlock, DETECT_MODES
         if not hasattr(_tls, 'pipeline_stack'):
             _tls.pipeline_stack = [Pipeline()]
 
@@ -234,6 +239,29 @@ class Pipeline(object):
             corr.orings = [oring]
             oring.owner = corr
             for b in (c, v):
+                self.blocks.remove(b)
+
+        # beamform -> detect -> reduce('time', nint): one BeamformBlock(detect=mode, nint=nint)
+        for bm in [b for b in self.blocks if isinstance(b, BeamformBlock) and b.fuse and b.detect is None]:
+            d = only_consumer(bm.orings[0])
+            if not (isinstance(d, DetectBlock) and d.fuse and d.mode in DETECT_MODES
+                    and d.specified_axis in (None, 'pol')):
+                continue
+            r = only_consumer(d.orings[0])
+            if not (isinstance(r, ReduceBlock) and r.fuse and r.specified_axis in ('time', 0) and r.op == 'sum'
+                    and isinstance(r.specified_factor, int) and r.specified_factor >= 2):
+                continue
+            iring, oring = bm.irings[0], r.orings[0]
+            _tls.pipeline_stack.append(self)
+            try:
+                fused = BeamformBlock(iring, bm.weights, detect=d.mode, nint=r.specified_factor,
+                                      gulp_nframe=bm.gulp_nframe, gpu=bm.gpu, core=bm.core)
+            finally:
+                _tls.pipeline_stack.pop()
+            iring.consumers.remove(bm)
+            fused.orings = [oring]
+            oring.owner = fused
+            for b in (bm, d, r):
                 self.blocks.remove(b)
 
     def shutdown(self):

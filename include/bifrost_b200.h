@@ -361,6 +361,28 @@ BFstatus bfLinAlgCorrelateCi4(BFlinalg handle, double alpha, BFarray const* a, B
                               double beta, BFarray const* c);
 BFstatus bfLinAlgCorrelateCi4ToStorage(BFlinalg handle, BFarray const* x, BFarray const* vis);
 
+/* Power beams in one pass: beamform, detect and integrate over time.  w and x
+ * are the a and b of the beamformer form of bfLinAlgMatMul (w [..., nb, K],
+ * x [..., K, ntime], batch dims broadcast as there); out is f32
+ * [..., nb/npb, nprod, ntime/nint] with any strides that are positive
+ * multiples of 4 bytes, and is only written.  mode is that of bfDetect:
+ * 0 scalar (npb 1, nprod 1), 2 stokes (2, 4), 3 stokes_i (2, 1),
+ * 4 coherence (2, 4); polarised modes take beam rows 2j and 2j+1 as the x and
+ * y polarisation of output beam j.  The result is, bit for bit,
+ *   bfLinAlgMatMul(handle, 1, w, x, 0, C)              C cf32 [..., nb, ntime]
+ *   bfDetect(C as [..., nb/npb, npb, ntime], D, mode, pol axis)
+ *   bfReduce(D, out, BF_REDUCE_SUM)                    over time, by nint
+ * (no reduce when nint = 1).  Operands the sm_90a beamformer takes (cf32 or
+ * ci16 w, ci4 or ci8 x, unit stride along K) run as one kernel that detects
+ * and integrates from registers; every other input runs the three calls
+ * through a workspace owned by the handle.  Returns BF_STATUS_UNSUPPORTED for
+ * jones or an unknown mode; BF_STATUS_INVALID_SHAPE for nint < 1,
+ * ntime % nint != 0, odd nb in a polarised mode or a wrong out shape;
+ * BF_STATUS_UNSUPPORTED_DTYPE for out not f32; otherwise what bfLinAlgMatMul
+ * returns for the same w and x. */
+BFstatus bfLinAlgBeamformDetect(BFlinalg handle, BFarray const* w, BFarray const* x,
+                                int mode, int nint, BFarray const* out);
+
 /* Host-only introspection of the FDMT plan bfFdmtInit would build (no device
  * needed).  step < 0: writes the number of steps to *nrow.  Otherwise writes
  * the row count of `step` to *nrow and, if rows != NULL, nrow triples

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -261,6 +261,9 @@ def main():
     if 'correlate_ci4' in ops:
         bench_correlate_ci4(stream, rng)
 
+    if 'beamform_detect' in ops:
+        bench_beamform_detect(stream, rng)
+
 
 def gpu_name():
     """Card name, power limit and max SM clock, read in the same run as the timings."""
@@ -420,6 +423,69 @@ def bench_beamform(stream, ref, rng):
                    max_abs_diff_vs_simt=float(np.abs(got - simt).max()))
             del d_w, d_c
         del d_x
+
+
+def bench_beamform_detect(stream, rng, nrep=10):
+    """Power beams, bfLinAlgBeamformDetect, against the three calls it
+    replaces (bfLinAlgMatMul into cf32 beams, bfDetect, bfReduce over time)
+    and the beamformer alone, timed alternately in the same loop: 512 chan,
+    K = 512, ntime 4096, cf32 weights, ci8 / ci4 voltages, nb dual-pol beam
+    rows, stokes and stokes_i, nint 16.  The fused and chain outputs are
+    compared bit for bit.  Bounds as bench_beamform: compulsory bytes
+    (voltages + weights + power beams) at 3.35 TB/s and 8 flops per complex
+    multiply-add at 67 TFLOP/s (H100 SXM data sheet, 700 W)."""
+    print(json.dumps({'op': 'beamform_detect.device', 'gpu': gpu_name()}), flush=True)
+    nchan, K, ntime, nint = 512, 512, 4096, 16
+    la = bf.linalg.LinAlg()
+    for xk in ('ci8', 'ci4'):
+        vb = 2 if xk == 'ci8' else 1
+        raw = rng.integers(0, 256, size=(ntime, nchan, K * vb), dtype=np.uint8)
+        xnp = raw.view(bf.DataType(xk).as_numpy_dtype()).reshape(ntime, nchan, K)
+        d_x = bf.asarray(bf.ndarray(xnp, dtype=xk), space='cuda')
+        del raw, xnp
+        xv = d_x.transpose((1, 2, 0))
+        for nb in (2, 8, 32, 64):
+            w = (rng.normal(size=(nchan, nb, K)) + 1j * rng.normal(size=(nchan, nb, K))).astype(np.complex64)
+            d_w = bf.asarray(w, space='cuda')
+            d_c = bf.empty((nchan, nb, ntime), 'cf32', 'cuda')
+            for mode in ('stokes', 'stokes_i'):
+                nprod = 4 if mode == 'stokes' else 1
+                d_d = bf.empty((nchan, nb // 2, nprod, ntime), 'f32', 'cuda')
+                d_f = bf.empty((nchan, nb // 2, nprod, ntime // nint), 'f32', 'cuda')
+                d_o = bf.empty((nchan, nb // 2, nprod, ntime // nint), 'f32', 'cuda')
+                cv = d_c.reshape(nchan, nb // 2, 2, ntime)
+                fns = {'fused': lambda: la.beamform_detect(d_w, xv, d_f, mode, nint),
+                       'chain': lambda: (la.matmul(1, d_w, xv, 0, d_c), bf.detect(cv, d_d, mode, 2),
+                                         bf.reduce(d_d, d_o, 'sum')),
+                       'beamform': lambda: la.matmul(1, d_w, xv, 0, d_c)}
+                for _ in range(2):
+                    for fn in fns.values():
+                        fn()
+                torch.cuda.synchronize()
+                times = {k: [] for k in fns}
+                for _ in range(nrep):
+                    for key, fn in fns.items():
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record(stream)
+                        fn()
+                        e1.record(stream)
+                        torch.cuda.synchronize()
+                        times[key].append(e0.elapsed_time(e1))
+                identical = bool(np.array_equal(np.asarray(d_f.copy('system')).view(np.uint32),
+                                                np.asarray(d_o.copy('system')).view(np.uint32)))
+                ms = {k: float(np.median(v)) for k, v in times.items()}
+                nbytes = ntime * nchan * K * vb + nchan * nb * K * 8 + nchan * (nb // 2) * nprod * (ntime // nint) * 4
+                flops = 8.0 * nchan * nb * K * ntime
+                t_hbm, t_fp = nbytes / 3.35e12 * 1e3, flops / 67e12 * 1e3
+                report('beamform_detect %s x cf32 %s nint=%d nb=%d nchan=%d K=%d ntime=%d'
+                       % (xk, mode, nint, nb, nchan, K, ntime), ms['fused'], nbytes,
+                       chain_ms=round(ms['chain'], 4), beamform_ms=round(ms['beamform'], 4),
+                       speedup_vs_chain=round(ms['chain'] / ms['fused'], 3),
+                       bound_by='HBM' if t_hbm >= t_fp else 'FP32', share_of_bound=round(max(t_hbm, t_fp) / ms['fused'], 3),
+                       identical=identical)
+                del d_d, d_f, d_o, cv
+            del d_w, d_c
+        del d_x, xv
 
 
 if __name__ == '__main__':
