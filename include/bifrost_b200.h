@@ -328,6 +328,29 @@ BFstatus bfVisibilitiesFillHermitian(BFarray const* in, BFarray const* out);
 BFstatus bfVisibilitiesToStorage(BFarray const* in, BFarray const* out);
 BFstatus bfVisibilitiesFromStorage(BFarray const* in, BFarray const* out);
 
+/* Boxcar pulse search of a dispersion bank (the FDMT's output).
+ * in  [..., ndm, ntime] f32, time unit stride, every other stride a multiple
+ *     of 4 bytes; leading (batch) dims are searched independently.
+ * out [..., ndm, nblk, 3] f32, last axis unit stride: (s, offset, width).
+ * Init: 1 <= nwidth <= 32 strictly increasing widths in [1, 4096] (host
+ * array), 1 <= decim <= 2^24.  With W the widest width, nout = ntime - W + 1
+ * starts (ntime >= W), nblk = ceil(nout / decim).  Per row and width,
+ * b_w[t] = sum_{k<w} x[t+k] for t < nout, and mu_w, sigma_w are the mean and
+ * population standard deviation of b_w over those starts (fp64).  Block j
+ * covers starts [j decim, min((j+1) decim, nout)); per width t_w is its first
+ * argmax of b_w, s_w = (b_w[t_w] - mu_w) / sigma_w (0 when sigma_w = 0), and
+ * the block reports the first width with the largest s_w as
+ * (s_w, t_w - j decim, w).  Deterministic: no atomics, fixed merge order.
+ * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
+ * (NULL, &size) query only, (ptr, &size) caller-provided. */
+typedef struct BFpulsesearch_impl* BFpulsesearch;
+
+BFstatus bfPulseSearchCreate(BFpulsesearch* plan);
+BFstatus bfPulseSearchInit(BFpulsesearch plan, int nwidth, int const* widths, int decim);
+BFstatus bfPulseSearchExecute(BFpulsesearch plan, BFarray const* in, BFarray const* out,
+                              void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfPulseSearchDestroy(BFpulsesearch plan);
+
 /* Correlate straight into the storage layout: x is [nchan, ntime, 2*nstand]
  * ci8 / ci16 / cf32 (the b of the b^H.b form of bfLinAlgMatMul, any strides
  * it takes, conjugated views honoured), vis is [nbaseline, nchan, 4] cf32 as

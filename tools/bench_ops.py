@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -264,6 +264,9 @@ def main():
     if 'beamform_detect' in ops:
         bench_beamform_detect(stream, rng)
 
+    if 'pulse_search' in ops:
+        bench_pulse_search(stream)
+
 
 def gpu_name():
     """Card name, power limit and max SM clock, read in the same run as the timings."""
@@ -486,6 +489,67 @@ def bench_beamform_detect(stream, rng, nrep=10):
                 del d_d, d_f, d_o, cv
             del d_w, d_c
         del d_x, xv
+
+
+def bench_pulse_search(stream, nrep=20):
+    """bfPulseSearchExecute on the config-2 bank: the 794 x 131072 f32 output
+    of the config-2 bfFdmtExecute (bench.make_input, made on the device),
+    widths 1..256 in powers of two, decim 256.  Timed alternately in the same
+    loop with a device-to-device copy of the bank and with the config-2
+    bfFdmtExecute itself.  The search reads the bank once and writes a peak
+    map nblk x 3 f32 per row; its HBM share is those bytes at 3.35 TB/s (H100
+    SXM data sheet, 700 W) over the time.  Two runs are compared bit for bit."""
+    import bench
+    print(json.dumps({'op': 'pulse_search.device', 'gpu': gpu_name()}), flush=True)
+    w = bench.workload(0)
+    d_in = bf.asarray(bench.make_input(w, 1), space='cuda')
+    md, ntime = w['max_delay'], w['ntime']
+    bank = bf.zeros((md, ntime), 'f32', 'cuda')
+    fplan = bf.fdmt.Fdmt()
+    fplan.init(w['nchan'], md, w['f0'], w['df'])
+    fplan.execute(d_in, bank)
+    bview = bank[:, :bench.NTIME_OUT]                         # the 131072 fully-summed samples of each row
+    widths, decim = [1 << k for k in range(9)], 256
+    nblk = bf.pulse_search.output_nblock(bench.NTIME_OUT, widths, decim)
+    plan = bf.pulse_search.PulseSearch()
+    plan.init(widths, decim)
+    d_a = bf.zeros((md, nblk, 3), 'f32', 'cuda')
+    d_b = bf.zeros((md, nblk, 3), 'f32', 'cuda')
+    nbytes_bank = md * bench.NTIME_OUT * 4
+    src = torch.empty(nbytes_bank, dtype=torch.uint8, device='cuda')
+    dst = torch.empty_like(src)
+    fbank = bf.zeros((md, ntime), 'f32', 'cuda')
+    fns = {'search': lambda: plan.execute(bview, d_a),
+           'copy': lambda: dst.copy_(src),
+           'fdmt': lambda: fplan.execute(d_in, fbank)}
+    for _ in range(3):
+        for fn in fns.values():
+            fn()
+    torch.cuda.synchronize()
+    times = {k: [] for k in fns}
+    for _ in range(nrep):
+        for key, fn in fns.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            fn()
+            e1.record(stream)
+            torch.cuda.synchronize()
+            times[key].append(e0.elapsed_time(e1))
+    plan.execute(bview, d_b)
+    torch.cuda.synchronize()
+    a, b = np.asarray(d_a.copy('system')), np.asarray(d_b.copy('system'))
+    ms = {k: float(np.median(v)) for k, v in times.items()}
+    nbytes = nbytes_bank + md * nblk * 3 * 4
+    top = np.argsort(a[..., 0].ravel())[::-1][:3]
+    report('pulse_search f32 %dx%d widths=1..256 decim=%d' % (md, bench.NTIME_OUT, decim), ms['search'], nbytes,
+           bank_GBps=round(nbytes_bank / ms['search'] / 1e6, 1),
+           hbm_share=round(nbytes / 3.35e12 * 1e3 / ms['search'], 3),
+           copy_ms=round(ms['copy'], 4), copy_GBps=round(2 * nbytes_bank / ms['copy'] / 1e6, 1),
+           fdmt_ms=round(ms['fdmt'], 4), search_over_fdmt=round(ms['search'] / ms['fdmt'], 3),
+           identical=bool(np.array_equal(a.view(np.uint32), b.view(np.uint32))),
+           top_peaks=[[int(i // nblk), int(i % nblk) * decim + int(a.reshape(-1, 3)[i, 1]),
+                       int(a.reshape(-1, 3)[i, 2]), round(float(a.reshape(-1, 3)[i, 0]), 2)] for i in top])
+    del d_in, bank, fbank, d_a, d_b, src, dst
 
 
 if __name__ == '__main__':
