@@ -351,6 +351,38 @@ BFstatus bfPulseSearchExecute(BFpulsesearch plan, BFarray const* in, BFarray con
                               void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfPulseSearchDestroy(BFpulsesearch plan);
 
+/* RFI excision by windowed spectral kurtosis (SK), for power filterbanks in
+ * front of the FDMT.
+ * x [..., ntime] u8, u16 or f32 power (i8 and every other dtype:
+ *   BF_STATUS_UNSUPPORTED_DTYPE); each leading index is one row (a channel),
+ *   time unit stride, every other stride and the base any multiple of the
+ *   item size.
+ * y same dtype and shape, its own leading strides, time unit stride; may be x
+ *   itself (same data and strides; any other overlap is undefined).
+ * sk NULL, or f32 [..., nwin] (last axis unit stride, other strides multiples
+ *   of 4 bytes): (float)sk per window.
+ * Init: 2 <= window M <= 2^20, nacc N >= 1 (raw spectra per sample), shape d
+ * finite and > 0 (1 for power from complex voltages), lo < hi both finite.
+ * Row r splits into nwin = ceil(ntime / M) windows of m samples (the last may
+ * be short).  S1 = sum x, S2 = sum x^2 (exact u64 sums for u8 / u16, fp64
+ * for f32); a = ((m N) d + 1) / (m - 1), sk = a ((m S2) / (S1 S1) - 1), each
+ * operation one fp64 rounding in this order.  A window is flagged unless
+ * lo <= sk <= hi (NaN, a constant, an all-zero or a one-sample window is
+ * flagged).  y = x on clean windows; on flagged ones the row's fill, the fp64
+ * sum of S1 over clean windows (ascending) over their sample count (0 if none),
+ * rounded to nearest even into the dtype.  Deterministic: no atomics.
+ * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
+ * (NULL, &size) query only, (ptr, &size) caller-provided.
+ * BF_STATUS_UNSUPPORTED_SHAPE when rows, rows x windows or ntime + M exceed
+ * 2^31 - 1. */
+typedef struct BFskflag_impl* BFskflag;
+
+BFstatus bfSkFlagCreate(BFskflag* plan);
+BFstatus bfSkFlagInit(BFskflag plan, int window, int nacc, double shape, double lo, double hi);
+BFstatus bfSkFlagExecute(BFskflag plan, BFarray const* x, BFarray const* y, BFarray const* sk,
+                         void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfSkFlagDestroy(BFskflag plan);
+
 /* Correlate straight into the storage layout: x is [nchan, ntime, 2*nstand]
  * ci8 / ci16 / cf32 (the b of the b^H.b form of bfLinAlgMatMul, any strides
  * it takes, conjugated views honoured), vis is [nbaseline, nchan, 4] cf32 as

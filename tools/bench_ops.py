@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -266,6 +266,12 @@ def main():
 
     if 'pulse_search' in ops:
         bench_pulse_search(stream)
+
+    if 'sk_flag' in ops:
+        bench_sk_flag(stream)
+
+    if 'sk_flag_kernels' in ops:
+        bench_sk_flag_kernels()
 
 
 def gpu_name():
@@ -550,6 +556,121 @@ def bench_pulse_search(stream, nrep=20):
            top_peaks=[[int(i // nblk), int(i % nblk) * decim + int(a.reshape(-1, 3)[i, 1]),
                        int(a.reshape(-1, 3)[i, 2]), round(float(a.reshape(-1, 3)[i, 0]), 2)] for i in top])
     del d_in, bank, fbank, d_a, d_b, src, dst
+
+
+def sk_flag_input(nrow, ntime, dtype, window, bad=0.03, seed=0):
+    """Gamma(4, 8) power drawn on the device (the sum of four exponentials),
+    with a `bad` share of its windows given four samples of +150, which sk
+    flags; returned as a bf device array of `dtype` ('u8' or 'f32')."""
+    g = torch.Generator(device='cuda').manual_seed(seed)
+    x = torch.zeros(nrow, ntime, device='cuda')
+    for _ in range(4):
+        x += torch.empty(nrow, ntime, device='cuda').exponential_(generator=g)
+    x *= 8
+    hit = torch.rand(nrow, ntime // window, 1, device='cuda', generator=g) < bad
+    x.view(nrow, ntime // window, window)[..., 100:104] += 150 * hit
+    x = torch.clamp(torch.round(x), 0, 255).to(torch.uint8) if dtype == 'u8' else x
+    d = bf.empty((nrow, ntime), dtype, 'cuda')
+    nbytes = x.numel() * x.element_size()
+    _check(_bf.bfMemcpy(d.ctypes.data, _bf.BF_SPACE_CUDA, x.data_ptr(), _bf.BF_SPACE_CUDA, nbytes))
+    bf.device.stream_synchronize()
+    return d
+
+
+SK_CASES = (('u8', 4096, 131072, 256, 4), ('f32', 4096, 32768, 256, 4))
+
+
+def bench_sk_flag(stream, nrep=20):
+    """bfSkFlagExecute on a u8 [4096, 131072] filterbank (the config-2 gulp),
+    window 256, nacc 4, out of place and in place, and on f32 [4096, 32768],
+    window 256, nacc 4.  Inputs are Gamma(4, 8) power with about 3 % of the windows
+    corrupted (sk_flag_input).  Each case is timed alternately in one loop
+    with a device-to-device copy of x.  Compulsory bytes: |x| + |y| out of
+    place, |x| + the flagged windows in place; their HBM share is those bytes
+    at 3.35 TB/s (H100 SXM data sheet, 700 W) over the time.  The in-place
+    case restores x from a pristine copy before every run (that copy is not
+    timed); two out-of-place runs are compared bit for bit."""
+    print(json.dumps({'op': 'sk_flag.device', 'gpu': gpu_name()}), flush=True)
+    for dt, nrow, ntime, M, N in SK_CASES:
+        isz = 1 if dt == 'u8' else 4
+        nbytes = nrow * ntime * isz
+        d_x = sk_flag_input(nrow, ntime, dt, M)
+        d_y = bf.empty((nrow, ntime), dt, 'cuda')
+        d_w = bf.empty((nrow, ntime), dt, 'cuda')
+        d_k = bf.empty((nrow, ntime // M), 'f32', 'cuda')
+        plan = bf.sk_flag.SkFlag()
+        plan.init(M, N)
+        src = torch.empty(nbytes, dtype=torch.uint8, device='cuda')
+        dst = torch.empty_like(src)
+
+        def restore():
+            _check(_bf.bfMemcpy(d_w.ctypes.data, _bf.BF_SPACE_CUDA, d_x.ctypes.data, _bf.BF_SPACE_CUDA, nbytes))
+        fns = {'out': (None, lambda: plan.execute(d_x, d_y)),
+               'copy': (None, lambda: dst.copy_(src))}
+        if dt == 'u8':
+            fns['inplace'] = (restore, lambda: plan.execute(d_w, d_w))
+        for _ in range(3):
+            for pre, fn in fns.values():
+                if pre:
+                    pre()
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in fns}
+        for _ in range(nrep):
+            for key, (pre, fn) in fns.items():
+                if pre:
+                    pre()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1))
+        y1 = np.asarray(d_y.copy('system'))
+        plan.execute(d_x, d_y, d_k)
+        bf.device.stream_synchronize()
+        y2, k = np.asarray(d_y.copy('system')), np.asarray(d_k.copy('system'))
+        lo, hi = plan.lo, plan.hi
+        flagged = float(np.mean(~((lo <= k) & (k <= hi))))
+        ms = {key: float(np.median(v)) for key, v in times.items()}
+        fields = dict(copy_ms=round(ms['copy'], 4), over_copy=round(ms['out'] / ms['copy'], 3),
+                      hbm_share=round(2 * nbytes / 3.35e12 * 1e3 / ms['out'], 3),
+                      flagged_share=round(flagged, 4), identical=bool(np.array_equal(y1, y2)))
+        if 'inplace' in ms:
+            inb = nbytes * (1 + flagged)
+            fields.update(inplace_ms=round(ms['inplace'], 4),
+                          inplace_hbm_share=round(inb / 3.35e12 * 1e3 / ms['inplace'], 3))
+        report('sk_flag %s %dx%d window=%d nacc=%d' % (dt, nrow, ntime, M, N), ms['out'], 2 * nbytes, **fields)
+        del d_x, d_y, d_w, d_k, src, dst
+
+
+def bench_sk_flag_kernels(nrep=10):
+    """Per-kernel device time of bfSkFlagExecute (out of place) on the
+    bench_sk_flag cases, from torch.profiler in a run of its own."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    print(json.dumps({'op': 'sk_flag_kernels.device', 'gpu': gpu_name()}), flush=True)
+    for dt, nrow, ntime, M, N in SK_CASES:
+        d_x = sk_flag_input(nrow, ntime, dt, M)
+        d_y = bf.empty((nrow, ntime), dt, 'cuda')
+        plan = bf.sk_flag.SkFlag()
+        plan.init(M, N)
+        for _ in range(3):
+            plan.execute(d_x, d_y)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(nrep):
+                plan.execute(d_x, d_y)
+            bf.device.stream_synchronize()
+            torch.cuda.synchronize()
+        per = {}
+        for e in prof.profiler.kineto_results.events():
+            if e.device_type() == DeviceType.CUDA and e.name().startswith('void bfb::sk_'):
+                name = e.name().split('<')[0].replace('void bfb::', '')
+                per.setdefault(name, []).append((e.end_ns() - e.start_ns()) / 1e6)
+        print(json.dumps(dict(op='sk_flag.kernels %s %dx%d window=%d' % (dt, nrow, ntime, M),
+                              **{k: round(float(np.median(v)), 4) for k, v in per.items()})), flush=True)
+        del d_x, d_y
 
 
 if __name__ == '__main__':
