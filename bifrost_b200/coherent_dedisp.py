@@ -1,0 +1,71 @@
+"""bf.coherent_dedisp.CoherentDedisp: coherent dedispersion of critically
+sampled complex baseband channels (extension, bfCoherentDedisp*;
+include/bifrost_b200.h).
+
+Each channel of x [nchan, ..., ntime] (ci4, ci8, ci16 or cf32 voltages) is
+filtered by overlap-save with N-point segments and the inverse of the
+cold-plasma transfer function, which aligns every output sample to the
+arrival time at its channel's top edge.  Output t depends on the input from
+t to t + overlap.  The output is cf32; integer inputs enter unscaled."""
+import ctypes
+import math
+
+from bifrost_b200.libbifrost import _bf, _check, _get, BifrostObject
+from bifrost_b200.ndarray import asarray
+
+KDM = 4.148741601e3          # MHz^2 pc^-1 cm^3 s
+NFFT_MIN, NFFT_MAX = 256, 1 << 20
+
+
+def dispersion_overlap(nchan, f0, df, dm):
+    """M: the dispersion smear of the worst channel in samples,
+    ceil(max_c D DM ((f_c - |df|/2)^-2 - (f_c + |df|/2)^-2) |df| 1e6) with
+    f_c = f0 + c df MHz.  0 at DM 0."""
+    adf = abs(float(df))
+    smear = 0.0
+    for c in range(int(nchan)):
+        fc = float(f0) + c * float(df)
+        lo, top = fc - 0.5 * adf, fc + 0.5 * adf
+        if lo <= 0:
+            raise ValueError("channel %d has its bottom edge at %g MHz" % (c, lo))
+        smear = max(smear, KDM * float(dm) * (1.0 / (lo * lo) - 1.0 / (top * top)) * adf * 1e6)
+    return int(math.ceil(smear))
+
+
+def default_nfft(overlap):
+    """The smallest power of two >= max(256, 4 overlap), which keeps at least
+    three quarters of every segment; ValueError above 2^20."""
+    n = NFFT_MIN
+    while n < 4 * int(overlap):
+        n *= 2
+    if n > NFFT_MAX:
+        raise ValueError("an overlap of %d samples needs nfft %d > 2^20" % (overlap, n))
+    return n
+
+
+class CoherentDedisp(BifrostObject):
+    def __init__(self):
+        BifrostObject.__init__(self, _bf.bfCoherentDedispCreate, _bf.bfCoherentDedispDestroy)
+
+    def init(self, nchan, f0, df, dm, nfft):
+        """Channels f0 + c df MHz (c < nchan), dispersion measure dm in
+        pc cm^-3, nfft-point segments."""
+        _check(_bf.bfCoherentDedispInit(self.obj, int(nchan), float(f0), float(df), float(dm), int(nfft)))
+        self.nchan, self.f0, self.df, self.dm, self.nfft = int(nchan), float(f0), float(df), float(dm), int(nfft)
+        self.overlap = int(_get(_bf.bfCoherentDedispGetOverlap, self.obj))
+
+    def execute(self, idata, odata):
+        """odata (cf32, idata's shape) = idata dedispersed."""
+        _check(_bf.bfCoherentDedispExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
+                                           None, None))
+        return odata
+
+    def get_workspace_size(self, idata, odata):
+        return _get(_bf.bfCoherentDedispExecute, self.obj, asarray(idata).as_BFarray(),
+                    asarray(odata).as_BFarray(), None)
+
+    def execute_workspace(self, idata, odata, workspace_ptr, workspace_size):
+        size = _bf.BFsize(workspace_size)
+        _check(_bf.bfCoherentDedispExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
+                                           workspace_ptr, ctypes.byref(size)))
+        return odata

@@ -1,0 +1,519 @@
+// coherent_dedisp.cu -- coherent dedispersion of critically sampled complex
+// baseband channels (extension, bfCoherentDedisp*; no reference counterpart).
+//
+// Channel c has centre f_c = f0 + c df MHz (df may be negative), top edge
+// f_top = f_c + |df|/2 and sample interval 1/|df| us.  With D = 4.148741601e3
+// MHz^2 pc^-1 cm^3 s, K = D DM 1e6, nu_k = fftfreq(N)[k] df and
+//   phi_k = sgn(df) K [nu_k (f_c^-2 - f_top^-2) - nu_k^2 / (f_c^2 (f_c + nu_k))]
+// cycles, H_k = exp(2 pi i phi_k) undoes the cold-plasma delay relative to
+// the channel's top edge.  Each row [.., ntime] of a channel is filtered by
+// overlap-save: segments start at s = 0, L, 2L, .. (L = N - M, M the worst
+// channel's smear in samples) while s < ntime, take N samples (zeros past
+// the end), and keep y[0 : min(L, ntime - s)] of y = IFFT(H . FFT(x)) / N.
+// Integer inputs enter as their integer values.  phi_k is evaluated in fp64
+// and reduced modulo one turn before it is rounded to fp32.
+//
+//   N <= 4096  coherent_dedisp_fused_kernel: one launch.  A CTA owns one
+//       channel, evaluates its chirp (with the 1/N folded in) into shared
+//       memory once, then loops over (row, segment) lines: load and convert
+//       N samples, forward radix-16 Stockham FFT (the fft_fast_kernel scheme,
+//       fft4096.cuh), multiply by H in registers, a second forward FFT of the
+//       conjugate (IFFT(z) = conj(FFT(conj z))), store the kept samples.
+//   N >= 8192  coherent_dedisp_gather_kernel (convert into [rows, nseg, N]
+//       cf32 segments in the workspace), forward bfFft in place,
+//       coherent_dedisp_chirp_kernel (times H / N), inverse bfFft in place,
+//       coherent_dedisp_keep_kernel (the kept L samples of each segment).
+//
+// Both paths take phi_k from cd_chirp.  No atomics: two runs give the same bits.
+#include "core.hpp"
+#include "fft4096.cuh"
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+
+namespace bfb {
+
+constexpr double CD_KDM   = 4.148741601e3;    // MHz^2 pc^-1 cm^3 s
+constexpr int    CD_NMIN  = 256;
+constexpr int    CD_NMAX  = 1 << 20;
+constexpr int    CD_NFUSE = 4096;             // longest transform of the fused kernel
+
+enum CdKind { CD_CF32 = 0, CD_CI8, CD_CI16, CD_CI4 };
+
+struct CdParams {
+	const char* in;               // bytes
+	float2*     out;              // cf32
+	int  nrowdim;                 // dims before time (axis 0 = channel)
+	long rshape[BF_MAX_DIMS];
+	long istride[BF_MAX_DIMS];    // bytes
+	long ostride[BF_MAX_DIMS];    // float2 elements
+	long ntime;
+	int  N, L;
+	long nseg;                    // segments per row
+	long nbatch;                  // rows per channel
+	double f0, df, K;
+	float2* ws;                   // long path: [rows][nseg][N]
+};
+
+// H_k / N = exp(2 pi i phi_k) / N for channel c: phi in fp64, reduced modulo
+// one turn before the rounding to fp32.
+__device__ __forceinline__ float2 cd_chirp(CdParams const& P, long c, int k) {
+	const double fc  = P.f0 + (double)c * P.df;
+	const double adf = fabs(P.df);
+	const double top = fc + 0.5 * adf;
+	const double nu  = (double)(k < P.N / 2 ? k : k - P.N) / (double)P.N * P.df;
+	double phi = P.K * (nu * (1.0 / (fc * fc) - 1.0 / (top * top)) - nu * nu / (fc * fc * (fc + nu)));
+	if( P.df < 0. ) phi = -phi;
+	phi -= rint(phi);
+	double s, co;
+	sincospi(2.0 * phi, &s, &co);
+	const double inv = 1.0 / (double)P.N;
+	return make_float2((float)(co * inv), (float)(s * inv));
+}
+
+template<int KIND>
+__device__ __forceinline__ float2 cd_load(const char* row, long t) {
+	if( KIND == CD_CF32 ) return ((const float2*)row)[t];
+	if( KIND == CD_CI8 )  { const char2 v = ((const char2*)row)[t]; return make_float2(v.x, v.y); }
+	if( KIND == CD_CI16 ) { const short2 v = ((const short2*)row)[t]; return make_float2(v.x, v.y); }
+	const signed char b = ((const signed char*)row)[t];          // high nibble real, low nibble imaginary
+	return make_float2((float)((signed char)(b & 0xF0) >> 4), (float)((signed char)(b << 4) >> 4));
+}
+
+__device__ __forceinline__ void cd_row_offsets(CdParams const& P, long r, long* io, long* oo) {
+	long a = 0, b = 0;
+	for( int d=P.nrowdim-1; d>=0; --d ) {
+		const long i = r % P.rshape[d];
+		r /= P.rshape[d];
+		a += i * P.istride[d];
+		b += i * P.ostride[d];
+	}
+	*io = a; *oo = b;
+}
+
+// --------------------------------------------------------------- fused path
+// Forward FFT of N = 256 R3 points across T = 16 R3 threads (fft_fast_kernel's
+// stages): thread p enters with x[p + T m] in v[m] and leaves with X[cd_index(s)]
+// in v[s].  tb: the twiddle bases, laid out as in fft_fast_kernel.
+template<int R3>
+__device__ __forceinline__ int cd_index(int p, int s) {
+	constexpr int T = 16 * R3, Q = 16 / R3;
+	if( R3 == 1 ) { const int k2 = p & 15; return (p - k2) * 16 + k2 + 16 * s; }
+	const int q = s / R3, t = s % R3;
+	const int j = p + T * q, k = j & 255;
+	(void)Q;
+	return (j - k) * R3 + k + 256 * t;
+}
+
+template<int R3>
+__device__ __forceinline__ void cd_fft(float (&vr)[16], float (&vi)[16], float2* buf,
+                                       const float2* tb, int tid, int p) {
+	constexpr int T = 16 * R3, Q = 16 / R3;
+	constexpr int LOG = (R3 == 16) ? 4 : (R3 == 8) ? 3 : (R3 == 4) ? 2 : (R3 == 2) ? 1 : 0;
+	// stage 1 (Ns = 1)
+	SDft<16>::apply(vr, vi);
+	__syncthreads();                              // previous readers of the buffer are done
+#pragma unroll
+	for( int t=0; t<16; ++t ) buf[spad(16 * p + t)] = make_float2(vr[t], vi[t]);
+	__syncthreads();
+	// stage 2 (Ns = 16)
+#pragma unroll
+	for( int m=0; m<16; ++m ) { float2 v = buf[spad(p + T * m)]; vr[m] = v.x; vi[m] = v.y; }
+	apply_twiddles(vr, vi, tb[tid], tb[256 + tid], tb[512 + tid], tb[768 + tid]);
+	SDft<16>::apply(vr, vi);
+	if( R3 == 1 ) return;
+	const int k2 = p & 15;
+	const int j0 = (p - k2) * 16 + k2;
+	__syncthreads();
+#pragma unroll
+	for( int t=0; t<16; ++t ) buf[spad(j0 + 16 * t)] = make_float2(vr[t], vi[t]);
+	__syncthreads();
+	// stage 3 (Ns = 256, radix R3): Q butterflies per thread
+#pragma unroll
+	for( int u=0; u<16; ++u ) { float2 v = buf[spad(p + T * u)]; vr[u] = v.x; vi[u] = v.y; }
+	float or_[16], oi_[16];
+#pragma unroll
+	for( int q=0; q<Q; ++q ) {
+		float ar[R3], ai[R3];
+#pragma unroll
+		for( int m=0; m<R3; ++m ) { ar[m] = vr[q + Q * m]; ai[m] = vi[q + Q * m]; }
+		fast_twiddle<R3>(ar, ai, tb + (4 + q * LOG) * 256 + tid);
+		SDft<R3>::apply(ar, ai);
+#pragma unroll
+		for( int t=0; t<R3; ++t ) { or_[q * R3 + t] = ar[t]; oi_[q * R3 + t] = ai[t]; }
+	}
+#pragma unroll
+	for( int s=0; s<16; ++s ) { vr[s] = or_[s]; vi[s] = oi_[s]; }
+}
+
+__device__ __forceinline__ float2 cd_twiddle(int k, int N) {      // exp(-2 pi i k / N)
+	double s, c;
+	sincospi(2.0 * (double)k / (double)N, &s, &c);
+	return make_float2((float)c, (float)-s);
+}
+
+template<int KIND, int R3>
+__global__ void __launch_bounds__(256, 2)
+coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
+	constexpr int N = 256 * R3, T = 16 * R3, G = 256 / T, Q = 16 / R3;
+	constexpr int LOG = (R3 == 16) ? 4 : (R3 == 8) ? 3 : (R3 == 4) ? 2 : (R3 == 2) ? 1 : 0;
+	constexpr int PITCH = N + (N >> 4) + 1;
+	extern __shared__ __align__(16) unsigned char cd_smem[];
+	float2* buf   = (float2*)cd_smem;
+	float2* tb    = buf + G * PITCH;                 // [4 + Q*LOG][256] twiddle bases
+	float2* chirp = tb + 12 * 256;                   // [N] H_k / N of this CTA's channel
+	const int tid = threadIdx.x, g = tid / T, p = tid % T;
+	buf += g * PITCH;
+	const long c = blockIdx.y;
+#pragma unroll
+	for( int i=0; i<4; ++i ) tb[i * 256 + tid] = cd_twiddle((R3 * ((p & 15) << i)) & (N - 1), N);
+#pragma unroll
+	for( int q=0; q<Q; ++q )
+#pragma unroll
+		for( int i=0; i<LOG; ++i ) tb[(4 + q * LOG + i) * 256 + tid] = cd_twiddle((((p + T * q) & 255) << i) & (N - 1), N);
+	for( int k=tid; k<N; k+=256 ) chirp[k] = cd_chirp(P, c, k);
+	// (the first barrier inside cd_fft publishes both tables)
+	const long nline = P.nbatch * P.nseg;
+	for( long L0 = (long)blockIdx.x * G; L0 < nline; L0 += (long)gridDim.x * G ) {
+		const long line = L0 + g;
+		const bool live = line < nline;
+		const long b = live ? line / P.nseg : 0;
+		const long t0 = live ? (line - b * P.nseg) * P.L : 0;
+		long io, oo;
+		cd_row_offsets(P, c * P.nbatch + b, &io, &oo);
+		const char* irow = P.in + io;
+		float vr[16], vi[16];
+#pragma unroll
+		for( int m=0; m<16; ++m ) {
+			const long t = t0 + p + T * m;
+			float2 v = make_float2(0.f, 0.f);
+			if( live && t < P.ntime ) v = cd_load<KIND>(irow, t);
+			vr[m] = v.x; vi[m] = v.y;
+		}
+		cd_fft<R3>(vr, vi, buf, tb, tid, p);
+		// z = conj(H X / N) into natural order for the second transform
+		__syncthreads();                          // every read of the last stage is done
+#pragma unroll
+		for( int s=0; s<16; ++s ) {
+			const int k = cd_index<R3>(p, s);
+			const float2 h = chirp[k];
+			buf[spad(k)] = make_float2(vr[s] * h.x - vi[s] * h.y, -(vr[s] * h.y + vi[s] * h.x));
+		}
+		__syncthreads();
+#pragma unroll
+		for( int m=0; m<16; ++m ) { const float2 v = buf[spad(p + T * m)]; vr[m] = v.x; vi[m] = v.y; }
+		cd_fft<R3>(vr, vi, buf, tb, tid, p);
+		if( live ) {
+			float2* orow = P.out + oo;
+			const long keep = min((long)P.L, P.ntime - t0);
+#pragma unroll
+			for( int s=0; s<16; ++s ) {
+				const int k = cd_index<R3>(p, s);
+				if( k < keep ) orow[t0 + k] = make_float2(vr[s], -vi[s]);
+			}
+		}
+	}
+}
+
+// ---------------------------------------------------------------- long path
+template<int KIND>
+__global__ void __launch_bounds__(256)
+coherent_dedisp_gather_kernel(const __grid_constant__ CdParams P, long nrows) {
+	const long total = nrows * P.nseg * P.N;
+	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
+		const int e = (int)(i % P.N);
+		const long rs = i / P.N;
+		const long r = rs / P.nseg, s = rs - r * P.nseg;
+		const long t = s * P.L + e;
+		float2 v = make_float2(0.f, 0.f);
+		if( t < P.ntime ) {
+			long io, oo;
+			cd_row_offsets(P, r, &io, &oo);
+			v = cd_load<KIND>(P.in + io, t);
+		}
+		P.ws[i] = v;
+	}
+}
+
+__global__ void __launch_bounds__(256)
+coherent_dedisp_chirp_kernel(const __grid_constant__ CdParams P, long nrows) {
+	const long total = nrows * P.nseg * P.N;
+	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
+		const int k = (int)(i % P.N);
+		const long r = i / P.N / P.nseg;
+		const float2 h = cd_chirp(P, r / P.nbatch, k);
+		const float2 x = P.ws[i];
+		P.ws[i] = make_float2(x.x * h.x - x.y * h.y, x.x * h.y + x.y * h.x);
+	}
+}
+
+__global__ void __launch_bounds__(256)
+coherent_dedisp_keep_kernel(const __grid_constant__ CdParams P, long nrows) {
+	const long total = nrows * P.ntime;
+	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
+		const long r = i / P.ntime, t = i - r * P.ntime;
+		const long s = t / P.L, e = t - s * P.L;
+		long io, oo;
+		cd_row_offsets(P, r, &io, &oo);
+		P.out[oo + t] = P.ws[(r * P.nseg + s) * P.N + e];
+	}
+}
+
+} // namespace bfb
+
+using namespace bfb;
+
+struct BFcoherentdedisp_impl {
+	bool   planned = false;
+	long   nchan = 0, nfft = 0, overlap = 0;
+	double f0 = 0., df = 0., dm = 0.;
+	BFfft  fft = nullptr;         // long path: one plan over [rows * nseg, N], run both ways
+	long   fft_lines = -1;
+	size_t fft_tmp = 0;
+	void*  own_ws = nullptr;
+	size_t own_size = 0;
+	~BFcoherentdedisp_impl() {
+		if( fft ) bfFftDestroy(fft);
+		if( own_ws ) cudaFree(own_ws);
+	}
+};
+
+namespace {
+
+constexpr size_t CD_ALIGN = 512;
+
+int cd_kind(BFdtype d) {
+	switch( d ) {
+	case BF_DTYPE_CF32: return CD_CF32;
+	case BF_DTYPE_CI8:  return CD_CI8;
+	case BF_DTYPE_CI16: return CD_CI16;
+	case BF_DTYPE_CI4:  return CD_CI4;
+	default:            return -1;
+	}
+}
+
+// [lines, N] cf32 view of the segment buffer (data filled in at execute time)
+BFarray cd_seg_array(void* data, long lines, long N) {
+	BFarray a = {};
+	a.data = data;
+	a.space = BF_SPACE_CUDA;
+	a.dtype = BF_DTYPE_CF32;
+	a.ndim = 2;
+	a.shape[0] = lines; a.shape[1] = N;
+	a.strides[0] = N * 8; a.strides[1] = 8;
+	return a;
+}
+
+// (Re)plans the long path's transform for `lines` segments; sets fft_tmp.
+BFstatus cd_plan_fft(BFcoherentdedisp plan, long lines) {
+	if( plan->fft && plan->fft_lines == lines ) return BF_STATUS_SUCCESS;
+	if( !plan->fft ) {
+		BFstatus s = bfFftCreate(&plan->fft);
+		if( s != BF_STATUS_SUCCESS ) return s;
+	}
+	BFarray a = cd_seg_array(nullptr, lines, plan->nfft);
+	int axis = 1;
+	size_t tmp = 0;
+	BFstatus s = bfFftInit(plan->fft, &a, &a, 1, &axis, 0, &tmp);
+	if( s != BF_STATUS_SUCCESS ) { plan->fft_lines = -1; return s; }
+	plan->fft_lines = lines;
+	plan->fft_tmp = tmp;
+	return BF_STATUS_SUCCESS;
+}
+
+template<int KIND>
+void cd_launch_fused(CdParams const& P, long nchan, cudaStream_t st) {
+	const int R3 = P.N / 256;
+	const int G = 256 / (16 * R3);
+	const size_t smem = ((size_t)G * (P.N + P.N / 16 + 1) + 12 * 256 + P.N) * sizeof(float2);
+	int nsm = 132;
+	int dev = 0;
+	if( cudaGetDevice(&dev) == cudaSuccess ) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+	// about eight CTAs per SM in all, split evenly over the channels: each CTA
+	// evaluates its channel's chirp once and loops over its share of the lines
+	const long groups = div_up(P.nbatch * P.nseg, (long)G);
+	const long per = std::max(1L, std::min(groups, div_up(8L * nsm, nchan)));
+	const dim3 grid((unsigned)per, (unsigned)nchan);
+#define BFB_CD_FUSED(R_) do { \
+		BFB_CUDA_THROW(cudaFuncSetAttribute(coherent_dedisp_fused_kernel<KIND, R_>, \
+			cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), BF_STATUS_INTERNAL_ERROR); \
+		coherent_dedisp_fused_kernel<KIND, R_><<<grid, 256, smem, st>>>(P); } while(0)
+	switch( R3 ) {
+	case 1:  BFB_CD_FUSED(1);  break;
+	case 2:  BFB_CD_FUSED(2);  break;
+	case 4:  BFB_CD_FUSED(4);  break;
+	case 8:  BFB_CD_FUSED(8);  break;
+	default: BFB_CD_FUSED(16); break;
+	}
+#undef BFB_CD_FUSED
+	count_launch();
+}
+
+unsigned cd_grid(long total) { return (unsigned)std::max(1L, std::min(div_up(total, 256L), 132L * 32)); }
+
+BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out,
+                    void* exec_storage, BFsize* exec_storage_size) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(in && out, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(plan->planned, BF_STATUS_INVALID_STATE);
+	BFB_ASSERT(space_on_device(in->space) && space_on_device(out->space), BF_STATUS_UNSUPPORTED_SPACE);
+	const int kind = cd_kind(in->dtype);
+	BFB_ASSERT(kind >= 0 && out->dtype == BF_DTYPE_CF32, BF_STATUS_UNSUPPORTED_DTYPE);
+	const int nd = in->ndim;
+	BFB_ASSERT(nd >= 2 && nd <= BF_MAX_DIMS && out->ndim == nd, BF_STATUS_INVALID_SHAPE);
+	for( int d=0; d<nd; ++d ) BFB_ASSERT(in->shape[d] == out->shape[d], BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(in->shape[0] == plan->nchan, BF_STATUS_INVALID_SHAPE);
+	const long isz = dtype_nbyte(in->dtype);
+	BFB_ASSERT(in->strides[nd-1] == isz && out->strides[nd-1] == 8, BF_STATUS_UNSUPPORTED_STRIDE);
+	BFB_ASSERT((uintptr_t)in->data % isz == 0 && (uintptr_t)out->data % 8 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	for( int d=0; d<nd-1; ++d )
+		BFB_ASSERT(in->strides[d] % isz == 0 && out->strides[d] % 8 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	const long ntime = in->shape[nd-1];
+	long nrows = 1;
+	for( int d=0; d<nd-1; ++d ) nrows *= in->shape[d];
+	const long nchan = plan->nchan;
+	BFB_ASSERT(nchan <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);      // channels run on gridDim.y
+	const long N = plan->nfft, L = N - plan->overlap;
+	const long nseg = div_up(ntime, L);
+	const bool fused = N <= CD_NFUSE;
+
+	size_t need = 0, seg_bytes = 0;
+	if( !fused && nrows * nseg > 0 ) {
+		seg_bytes = round_up<size_t>((size_t)(nrows * nseg * N) * 8, CD_ALIGN);
+		BFstatus s = cd_plan_fft(plan, nrows * nseg);
+		if( s != BF_STATUS_SUCCESS ) return s;
+		need = seg_bytes + round_up<size_t>(plan->fft_tmp, CD_ALIGN);
+	}
+	need = std::max(need, CD_ALIGN);
+	if( exec_storage_size ) {
+		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
+		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
+	} else {
+		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
+		if( plan->own_size < need ) {
+			if( plan->own_ws ) cudaFree(plan->own_ws);
+			plan->own_ws = nullptr; plan->own_size = 0;
+			BFB_CUDA(cudaMalloc(&plan->own_ws, need), BF_STATUS_MEM_ALLOC_FAILED);
+			plan->own_size = need;
+		}
+		exec_storage = plan->own_ws;
+	}
+	if( nrows == 0 || ntime == 0 ) return BF_STATUS_SUCCESS;
+
+	CdParams P = {};
+	P.in  = (const char*)in->data;
+	P.out = (float2*)out->data;
+	P.nrowdim = nd - 1;
+	for( int d=0; d<nd-1; ++d ) {
+		P.rshape[d]  = in->shape[d];
+		P.istride[d] = in->strides[d];
+		P.ostride[d] = out->strides[d] / 8;
+	}
+	P.ntime  = ntime;
+	P.N      = (int)N;
+	P.L      = (int)L;
+	P.nseg   = nseg;
+	P.nbatch = nrows / nchan;
+	P.f0 = plan->f0;
+	P.df = plan->df;
+	P.K  = CD_KDM * plan->dm * 1e6;
+	cudaStream_t st = thread_stream();
+	if( fused ) {
+		switch( kind ) {
+		case CD_CF32: cd_launch_fused<CD_CF32>(P, nchan, st); break;
+		case CD_CI8:  cd_launch_fused<CD_CI8>(P, nchan, st);  break;
+		case CD_CI16: cd_launch_fused<CD_CI16>(P, nchan, st); break;
+		default:      cd_launch_fused<CD_CI4>(P, nchan, st);  break;
+		}
+		BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+		return BF_STATUS_SUCCESS;
+	}
+	P.ws = (float2*)exec_storage;
+	void* tmp = (char*)exec_storage + seg_bytes;
+	const long nws = nrows * nseg * N;
+	switch( kind ) {
+	case CD_CF32: coherent_dedisp_gather_kernel<CD_CF32><<<cd_grid(nws), 256, 0, st>>>(P, nrows); break;
+	case CD_CI8:  coherent_dedisp_gather_kernel<CD_CI8><<<cd_grid(nws), 256, 0, st>>>(P, nrows);  break;
+	case CD_CI16: coherent_dedisp_gather_kernel<CD_CI16><<<cd_grid(nws), 256, 0, st>>>(P, nrows); break;
+	default:      coherent_dedisp_gather_kernel<CD_CI4><<<cd_grid(nws), 256, 0, st>>>(P, nrows);  break;
+	}
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	const BFarray seg = cd_seg_array(P.ws, nrows * nseg, N);
+	BFstatus s = bfFftExecute(plan->fft, &seg, &seg, 0, tmp, plan->fft_tmp);
+	if( s != BF_STATUS_SUCCESS ) return s;
+	coherent_dedisp_chirp_kernel<<<cd_grid(nws), 256, 0, st>>>(P, nrows);
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	s = bfFftExecute(plan->fft, &seg, &seg, 1, tmp, plan->fft_tmp);
+	if( s != BF_STATUS_SUCCESS ) return s;
+	coherent_dedisp_keep_kernel<<<cd_grid(nrows * ntime), 256, 0, st>>>(P, nrows);
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	return BF_STATUS_SUCCESS;
+}
+
+} // namespace
+
+extern "C" {
+
+BFstatus bfCoherentDedispCreate(BFcoherentdedisp* plan_ptr) {
+	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
+	*plan_ptr = nullptr;
+	BFB_TRY(*plan_ptr = new BFcoherentdedisp_impl());
+	return BF_STATUS_SUCCESS;
+}
+
+BFstatus bfCoherentDedispInit(BFcoherentdedisp plan, BFsize nchan, double f0, double df,
+                              double dm, BFsize nfft) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(nchan > 0 && nchan <= (BFsize)INT_MAX, BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(std::isfinite(f0) && std::isfinite(df) && std::isfinite(dm), BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(dm >= 0. && df != 0., BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(nfft >= (BFsize)CD_NMIN && nfft <= (BFsize)CD_NMAX && (nfft & (nfft - 1)) == 0,
+	           BF_STATUS_INVALID_ARGUMENT);
+	const double adf = std::fabs(df);
+	// M = ceil(max_c D DM ((f_c - |df|/2)^-2 - (f_c + |df|/2)^-2) |df| 1e6)
+	double smear = 0.;
+	for( BFsize c=0; c<nchan; ++c ) {
+		const double fc = f0 + (double)c * df;
+		const double lo = fc - 0.5 * adf, top = fc + 0.5 * adf;
+		BFB_ASSERT(lo > 0., BF_STATUS_INVALID_ARGUMENT);
+		const double d = CD_KDM * dm * (1.0 / (lo * lo) - 1.0 / (top * top)) * adf * 1e6;
+		smear = std::max(smear, d);
+	}
+	BFB_ASSERT(std::isfinite(smear), BF_STATUS_INVALID_ARGUMENT);
+	const double M = std::ceil(smear);
+	BFB_ASSERT(M < (double)nfft, BF_STATUS_INVALID_ARGUMENT);
+	plan->nchan   = (long)nchan;
+	plan->f0      = f0;
+	plan->df      = df;
+	plan->dm      = dm;
+	plan->nfft    = (long)nfft;
+	plan->overlap = (long)M;
+	plan->fft_lines = -1;
+	plan->planned = true;
+	return BF_STATUS_SUCCESS;
+}
+
+BFstatus bfCoherentDedispGetOverlap(BFcoherentdedisp plan, BFsize* noverlap) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(noverlap, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(plan->planned, BF_STATUS_INVALID_STATE);
+	*noverlap = (BFsize)plan->overlap;
+	return BF_STATUS_SUCCESS;
+}
+
+BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out,
+                                 void* exec_storage, BFsize* exec_storage_size) {
+	BFB_TRY(return cd_execute(plan, in, out, exec_storage, exec_storage_size));
+}
+
+BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	delete plan;
+	return BF_STATUS_SUCCESS;
+}
+
+} // extern "C"

@@ -531,26 +531,6 @@ fft_regs_kernel(const __grid_constant__ FftPass<float> P) {
 	}
 }
 
-// v[m] *= w^m, m = 1..R-1, from the tabulated powers w^(2^i) (R = 2, 4, 8, 16).
-template<int R>
-__device__ __forceinline__ void fast_twiddle(float (&ar)[R], float (&ai)[R], const float2* __restrict__ tbq) {
-	float2 w[R];
-#pragma unroll
-	for( int i=0; (1 << i) < R; ++i ) w[1 << i] = tbq[i * 256];
-#pragma unroll
-	for( int m=3; m<R; ++m ) {
-		if( (m & (m - 1)) == 0 ) continue;                  // powers of two come from the table
-		const int hi = (m >= 8) ? 8 : (m >= 4) ? 4 : 2;     // m = hi + rest, rest < hi
-		w[m] = cmulf(w[m - hi], w[hi]);
-	}
-#pragma unroll
-	for( int m=1; m<R; ++m ) {
-		float tr = ar[m] * w[m].x - ai[m] * w[m].y;
-		ai[m] = ar[m] * w[m].y + ai[m] * w[m].x;
-		ar[m] = tr;
-	}
-}
-
 // Contiguous c2c transforms of length N = 256 * R3 (256 .. 4096): 16 points per
 // thread, N/16 threads per line, 256/(N/16) lines per CTA, radix 16 x 16 x R3
 // Stockham stages through padded interleaved shared memory (same scheme as

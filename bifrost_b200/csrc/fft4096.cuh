@@ -1,6 +1,6 @@
 // fft4096.cuh -- the 4096-point forward FFT core shared by the fused
-// spectrometer kernel (spectrometer.cu) and the contiguous fast path of bfFft
-// (fft.cu): 256 threads, 16 points per thread, three radix-16 Stockham stages,
+// spectrometer kernel (spectrometer.cu), the contiguous fast path of bfFft
+// (fft.cu) and the fused coherent dedispersion kernel (coherent_dedisp.cu):256 threads, 16 points per thread, three radix-16 Stockham stages,
 // interleaved-complex shared memory with one pad slot per 16 points, twiddles
 // from four exactly tabulated powers per stage.
 #pragma once
@@ -73,6 +73,28 @@ __device__ __forceinline__ void apply_twiddles(float (&vr)[16], float (&vi)[16],
 		float tr = vr[t] * w[t].x - vi[t] * w[t].y;
 		vi[t] = vr[t] * w[t].y + vi[t] * w[t].x;
 		vr[t] = tr;
+	}
+}
+
+// v[m] *= w^m, m = 1..R-1, from the tabulated powers w^(2^i) (R = 2, 4, 8, 16);
+// the last, radix-R3 stage of fft_fast_kernel (fft.cu) and of the coherent
+// dedispersion kernel (coherent_dedisp.cu).
+template<int R>
+__device__ __forceinline__ void fast_twiddle(float (&ar)[R], float (&ai)[R], const float2* __restrict__ tbq) {
+	float2 w[R];
+#pragma unroll
+	for( int i=0; (1 << i) < R; ++i ) w[1 << i] = tbq[i * 256];
+#pragma unroll
+	for( int m=3; m<R; ++m ) {
+		if( (m & (m - 1)) == 0 ) continue;                  // powers of two come from the table
+		const int hi = (m >= 8) ? 8 : (m >= 4) ? 4 : 2;     // m = hi + rest, rest < hi
+		w[m] = cmulf(w[m - hi], w[hi]);
+	}
+#pragma unroll
+	for( int m=1; m<R; ++m ) {
+		float tr = ar[m] * w[m].x - ai[m] * w[m].y;
+		ai[m] = ar[m] * w[m].y + ai[m] * w[m].x;
+		ar[m] = tr;
 	}
 }
 

@@ -290,10 +290,26 @@ class ViewRing(object):
         shape[fax] = (data.nbytes * 8) // (known * dt.itemsize_bits)
         if list(data.shape) == shape and data.bf.dtype == dt:
             return data
+        strides = None
         if not data.flags['C_CONTIGUOUS']:
-            raise ValueError("Header views need C-contiguous spans")
-        return ndarray(space=data.bf.space, buffer=data.ctypes.data, shape=shape, dtype=dt,
+            strides = _view_strides(data, shape) if data.bf.dtype == dt else None
+            if strides is None:
+                raise ValueError("Header views need C-contiguous spans")
+        return ndarray(space=data.bf.space, buffer=data.ctypes.data, shape=shape, dtype=dt, strides=strides,
                        native=data.bf.native, conjugated=data.bf.conjugated)
+
+
+def _view_strides(data, shape):
+    """Strides that present the strided span `data` with `shape` without a copy
+    (e.g. axes merged inside a ringlet, after a transpose that left the frame
+    axis inside), or None if there are none.  Found by numpy's no-copy reshape
+    of a probe with data's strides that never touches the memory."""
+    probe = np.lib.stride_tricks.as_strided(np.zeros(1, np.dtype((np.void, data.itemsize))),
+                                            shape=data.shape, strides=data.strides)
+    try:
+        return np.reshape(probe, shape, copy=False).strides
+    except ValueError:
+        return None
 
 
 class Reader(object):

@@ -383,6 +383,46 @@ BFstatus bfSkFlagExecute(BFskflag plan, BFarray const* x, BFarray const* y, BFar
                          void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfSkFlagDestroy(BFskflag plan);
 
+/* Coherent dedispersion (extension; no reference counterpart): removes the
+ * cold-plasma dispersion inside each critically sampled complex channel of
+ * baseband voltages, ahead of detection.
+ * Channel c has centre f_c = f0 + c df MHz (df may be negative: the spectrum
+ * inside each channel is then inverted too), top edge f_top = f_c + |df|/2 and
+ * sample interval 1/|df| us.  With D = 4.148741601e3 MHz^2 pc^-1 cm^3 s:
+ *   M = ceil(max_c D DM ((f_c - |df|/2)^-2 - f_top^-2) |df| 1e6)  (the overlap;
+ *       0 at DM 0), K = D DM 1e6, nu_k = fftfreq(N)[k] df MHz,
+ *   phi_k = sgn(df) K [nu_k (f_c^-2 - f_top^-2) - nu_k^2 / (f_c^2 (f_c + nu_k))]
+ *       cycles, H_k = exp(2 pi i phi_k) (numpy's forward sign convention).
+ * H undoes the delay D DM (f^-2 - f_top^-2) of sky frequency f = f_c + nu, so
+ * output sample t is aligned to the arrival time at its channel's top edge
+ * and depends on the input from t to t + M only.  Each row is filtered by
+ * overlap-save: segments start at s = 0, L, 2L, .. (L = N - M) while
+ * s < ntime, take N samples (zeros past the end of the row) and write
+ * y[0 : min(L, ntime - s)] of y = IFFT(H . FFT(x_seg)) / N to out[s : ..].
+ * Outputs t >= ntime - M see those zeros.  Integer inputs enter as their
+ * integer values (ci4 high nibble real), unscaled.  phi is evaluated in fp64
+ * and reduced modulo one turn before rounding to fp32.
+ * Init: BF_STATUS_INVALID_ARGUMENT unless nchan > 0, every argument finite,
+ * DM >= 0, df != 0, every channel's bottom edge > 0 MHz, nfft a power of two
+ * in [256, 2^20] and M < nfft.  Host work only.
+ * in [nchan, ..., ntime] ci4 / ci8 / ci16 / cf32 in device space (axis 0 the
+ *   channel, the axes between are batch axes), time unit stride, every other
+ *   stride and the base any multiple of the item size.
+ * out cf32, same shape, time unit stride; only written; must not overlap in.
+ * N <= 4096 runs one fused kernel; longer N run bfFft through plans the
+ * handle owns.  Deterministic: no atomics.  exec_storage follows the FDMT's
+ * protocol: (NULL, NULL) library-managed, (NULL, &size) query only,
+ * (ptr, &size) caller-provided. */
+typedef struct BFcoherentdedisp_impl* BFcoherentdedisp;
+
+BFstatus bfCoherentDedispCreate(BFcoherentdedisp* plan);
+BFstatus bfCoherentDedispInit(BFcoherentdedisp plan, BFsize nchan, double f0, double df,
+                              double dm, BFsize nfft);
+BFstatus bfCoherentDedispGetOverlap(BFcoherentdedisp plan, BFsize* noverlap);
+BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out,
+                                 void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan);
+
 /* Correlate straight into the storage layout: x is [nchan, ntime, 2*nstand]
  * ci8 / ci16 / cf32 (the b of the b^H.b form of bfLinAlgMatMul, any strides
  * it takes, conjugated views honoured), vis is [nbaseline, nchan, 4] cf32 as

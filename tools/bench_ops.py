@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -272,6 +272,9 @@ def main():
 
     if 'sk_flag_kernels' in ops:
         bench_sk_flag_kernels()
+
+    if 'coherent_dedisp' in ops:
+        bench_coherent_dedisp(stream)
 
 
 def gpu_name():
@@ -673,5 +676,112 @@ def bench_sk_flag_kernels(nrep=10):
         del d_x, d_y
 
 
+CD_CASES = ((100., 4096), (1000., 65536))            # (DM, nfft): one case on each kernel path
+
+
+def bench_coherent_dedisp(stream, nrep=10):
+    """bfCoherentDedispExecute on ci8 [64 chan, 2 pol, 2^20 + M] (0.67 s of a
+    100 MHz band: f0 = 1300.78125 MHz, df = 1.5625 MHz) at DM 100 (M = 921,
+    N = 4096, fused kernel) and DM 1000 (M = 9204, N = 65536, bfFft path).
+    Timed alternately in one loop with: the same filter from today's public
+    calls at the same N on pre-gathered cf32 segments (bfFft forward, bfMap
+    times a precomputed cf32 chirp, bfFft inverse); cuFFT through torch.fft on
+    the same segments (bench tooling only); a device-to-device copy of the
+    output bytes.  Compulsory bytes per sample: 2 N / L (ci8 read N / L times)
+    + 8 (cf32 written); their HBM share is those bytes at 3.35 TB/s (H100 SXM
+    data sheet, 700 W) over the time.  FP32 work: 2 x 5 N log2 N / L flop per
+    sample.  Every pair of outputs is compared on the kept samples: max |a - b|
+    over max |b| per row."""
+    from oracle import coherent_dedisp as ocd
+    print(json.dumps({'op': 'coherent_dedisp.device', 'gpu': gpu_name()}), flush=True)
+    nchan, npol, f0, df = 64, 2, 1300.78125, 1.5625
+    for dm, n in CD_CASES:
+        m = ocd.overlap(nchan, f0, df, dm)
+        L = n - m
+        ntime = (1 << 20) + m
+        nseg = -(-ntime // L)
+        rows = nchan * npol
+        g = torch.Generator(device='cuda').manual_seed(1)
+        raw = torch.randint(-127, 128, (nchan, npol, ntime, 2), dtype=torch.int8, device='cuda', generator=g)
+        d_x = bf.empty((nchan, npol, ntime), 'ci8', 'cuda')
+        _check(_bf.bfMemcpy(d_x.ctypes.data, _bf.BF_SPACE_CUDA, raw.data_ptr(), _bf.BF_SPACE_CUDA, raw.numel()))
+        d_y = bf.empty((nchan, npol, ntime), 'cf32', 'cuda')
+        plan = bf.coherent_dedisp.CoherentDedisp()
+        plan.init(nchan, f0, df, dm, n)
+        # cf32 segments [rows, nseg, N] (zeros past the end) and the chirp with 1/N folded in
+        xc = torch.view_as_complex(raw.float()).reshape(rows, ntime)
+        xp = torch.zeros(rows, (nseg - 1) * L + n, dtype=torch.complex64, device='cuda')
+        xp[:, :ntime] = xc
+        seg = xp.unfold(1, n, L).contiguous()
+        del xp, xc
+        h = np.stack([ocd.chirp(n, f0 + c * df, df, dm) / n for c in range(nchan)])
+        h_t = torch.from_numpy(np.repeat(h, npol, axis=0).astype(np.complex64)).cuda()
+        d_src = bf.empty((rows, nseg, n), 'cf32', 'cuda')
+        _check(_bf.bfMemcpy(d_src.ctypes.data, _bf.BF_SPACE_CUDA, seg.data_ptr(), _bf.BF_SPACE_CUDA,
+                            rows * nseg * n * 8))
+        d_seg = bf.empty((rows, nseg, n), 'cf32', 'cuda')
+        d_h = bf.empty((rows, n), 'cf32', 'cuda')
+        _check(_bf.bfMemcpy(d_h.ctypes.data, _bf.BF_SPACE_CUDA, h_t.data_ptr(), _bf.BF_SPACE_CUDA, rows * n * 8))
+        fft = bf.fft.Fft()
+        fft.init(d_src, d_seg, axes=[2])
+
+        def composed():
+            fft.execute(d_src, d_seg, inverse=False)
+            bf.map("y(r,s,k) = y(r,s,k) * h(r,k)", {'y': d_seg, 'h': d_h}, axis_names=('r', 's', 'k'),
+                   shape=d_seg.shape)
+            fft.execute(d_seg, d_seg, inverse=True)
+        t_out = {}
+
+        def torchfft():
+            t_out['y'] = torch.fft.ifft(torch.fft.fft(seg, dim=2) * h_t[:, None, :], dim=2, norm='forward')
+        nbytes_out = rows * ntime * 8
+        src = torch.empty(nbytes_out, dtype=torch.uint8, device='cuda')
+        dst = torch.empty_like(src)
+        fns = {'new': lambda: plan.execute(d_x, d_y), 'composed': composed, 'torch': torchfft,
+               'copy': lambda: dst.copy_(src)}
+        for _ in range(2):
+            for fn in fns.values():
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in fns}
+        for _ in range(nrep):
+            for key, fn in fns.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1))
+        # kept samples of every output, [rows, ntime]
+        y_new = np.asarray(d_y.copy('system')).reshape(rows, ntime)
+        plan.execute(d_x, d_y)
+        bf.device.stream_synchronize()
+        identical = bool(np.array_equal(y_new.view(np.uint64),
+                                        np.asarray(d_y.copy('system')).reshape(rows, ntime).view(np.uint64)))
+        y_cmp = np.asarray(d_seg.copy('system'))[:, :, :L].reshape(rows, nseg * L)[:, :ntime]
+        y_tor = t_out['y'][:, :, :L].reshape(rows, nseg * L)[:, :ntime].cpu().numpy()
+
+        def maxrel(a, b):
+            return float(max(np.abs(a[r] - b[r]).max() / np.abs(b[r]).max() for r in range(rows)))
+        ms = {key: float(np.median(v)) for key, v in times.items()}
+        per_sample = 2.0 * n / L + 8
+        nsamp = rows * ntime
+        flop = 2 * 5 * n * np.log2(n) / L
+        report('coherent_dedisp ci8 %dx%dx%d DM=%g N=%d M=%d' % (nchan, npol, ntime, dm, n, m), ms['new'],
+               per_sample * nsamp,
+               path='fused' if n <= 4096 else 'bfFft',
+               realtime=round(ntime / (df * 1e6) / (ms['new'] * 1e-3), 1),
+               hbm_share=round(per_sample * nsamp / 3.35e12 * 1e3 / ms['new'], 3),
+               compulsory_GB=round(per_sample * nsamp / 1e9, 3),
+               flop_per_sample=round(flop, 1), fp32_TFLOPs=round(flop * nsamp / ms['new'] / 1e9, 2),
+               composed_ms=round(ms['composed'], 4), torch_fft_ms=round(ms['torch'], 4),
+               copy_ms=round(ms['copy'], 4),
+               err_new_vs_composed=maxrel(y_new, y_cmp), err_new_vs_torch=maxrel(y_new, y_tor),
+               err_composed_vs_torch=maxrel(y_cmp, y_tor), identical=identical)
+        del d_x, d_y, d_src, d_seg, d_h, seg, raw, h_t, src, dst, t_out, fft, plan
+        torch.cuda.empty_cache()
+
+
 if __name__ == '__main__':
     main()
+
