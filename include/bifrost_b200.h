@@ -423,6 +423,46 @@ BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarr
                                  void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan);
 
+/* Pulsar folding (extension; no reference counterpart): phase-binned profiles
+ * of a topocentric spin model.
+ * in    [nchan, ..., ntime] u8 / u16 / f32 in device space, time unit stride,
+ *       every other stride and the base any multiple of the item size.  A row
+ *       is any index of the leading axes; its channel c is the first index.
+ * out   [nchan, ..., nbin] f32, bin unit stride, other strides multiples of 4
+ *       bytes: the per-row sums.
+ * count [nchan, nbin] i32, bin unit stride: the samples of channel c in each
+ *       bin (they do not depend on the other leading axes).
+ * Init: 1 <= nbin <= 4096, nchan >= 1, tsamp > 0 s, nu > 0 Hz, t0 (the time
+ * of stream sample 0 at the reference frequency, s from the ephemeris epoch),
+ * nudot, nuddot and every delays[c] (s, host array of nchan) finite:
+ * otherwise BF_STATUS_INVALID_ARGUMENT; delays NULL: BF_STATUS_INVALID_POINTER.
+ * Host work only.  With `first` the stream index of in's sample 0, sample t of
+ * channel c goes to bin
+ *   a_c  = t0 - delay[c]
+ *   tau  = a_c + (double)(first + t) * tsamp
+ *   phi  = ((c3 tau + c2) tau + nu) tau       c2 = 0.5 nudot, c3 = nuddot / 6.0
+ *   frac = phi - floor(phi)
+ *   bin  = min((int)floor(frac * nbin), nbin - 1)
+ * every step one fp64 operation rounded to nearest (no FMA), so splitting a
+ * stream into calls of any length bins every sample as one call would.  Each
+ * call's contribution to (row, bin) is summed in fp64 (exact for u8 / u16; in
+ * the kernel's fixed order for f32, so two runs give the same bits); with
+ * accumulate = 0, out = (float)partial and count = n; with accumulate = 1,
+ * out = (float)((double)out + partial) and count += n.  A NaN or inf sample
+ * poisons only its own bin.  Counts must stay below 2^31.
+ * BF_STATUS_UNSUPPORTED_SHAPE when rows or ntime exceed 32 bits.  ntime = 0
+ * or no rows is a no-op that, with accumulate = 0, still zeroes out and count.
+ * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
+ * (NULL, &size) query only, (ptr, &size) caller-provided. */
+typedef struct BFfold_impl* BFfold;
+
+BFstatus bfFoldCreate(BFfold* plan);
+BFstatus bfFoldInit(BFfold plan, int nbin, BFsize nchan, double const* delays, double tsamp,
+                    double t0, double nu, double nudot, double nuddot);
+BFstatus bfFoldExecute(BFfold plan, BFarray const* in, BFoffset first, BFarray const* out,
+                       BFarray const* count, int accumulate, void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfFoldDestroy(BFfold plan);
+
 /* Correlate straight into the storage layout: x is [nchan, ntime, 2*nstand]
  * ci8 / ci16 / cf32 (the b of the b^H.b form of bfLinAlgMatMul, any strides
  * it takes, conjugated views honoured), vis is [nbaseline, nchan, 4] cf32 as

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -275,6 +275,9 @@ def main():
 
     if 'coherent_dedisp' in ops:
         bench_coherent_dedisp(stream)
+
+    if 'fold' in ops:
+        bench_fold(stream)
 
 
 def gpu_name():
@@ -779,6 +782,98 @@ def bench_coherent_dedisp(stream, nrep=10):
                err_new_vs_composed=maxrel(y_new, y_cmp), err_new_vs_torch=maxrel(y_new, y_tor),
                err_composed_vs_torch=maxrel(y_cmp, y_tor), identical=identical)
         del d_x, d_y, d_src, d_seg, d_h, seg, raw, h_t, src, dst, t_out, fft, plan
+        torch.cuda.empty_cache()
+
+
+FOLD_FP64_OPS = 11          # fp64 operations per sample in the phase and bin (DESIGN section 8)
+FOLD_FP64_RATE = 16.7e12    # fp64 operations / s: 132 SMs x 64 FP64 lanes x 1.98 GHz (H100 SXM, 700 W)
+
+
+def bench_fold(stream, nrep=10):
+    """bfFoldExecute on three inputs: f32 [64, 4, 2^20] at nbin 1024, nu 641.9
+    Hz, tsamp 0.64 us (Stokes from the coherent chain; channels 1300.78125 +
+    1.5625 c MHz, top-edge delays at DM 100), and u8 [4096, 131072] at nbin
+    256, tsamp 64 us (a config-2 filterbank, 1500 MHz down to 1200 MHz, DM
+    100) with nu 1.4 Hz and 300 Hz.  Timed alternately in one loop with the
+    same fold composed in torch (fp64 bins, then scatter_add_ of f32 into
+    [rows, nbin]; bench tooling only) and a device-to-device copy of the
+    input.  Bounds: the input bytes at 3.35 TB/s, and FOLD_FP64_OPS fp64
+    operations per sample at FOLD_FP64_RATE (H100 SXM data sheet, 700 W).
+    Counts are compared exactly with the torch composition, sums to 1e-5 of
+    the bin's magnitude, and two runs bit for bit."""
+    print(json.dumps({'op': 'fold.device', 'gpu': gpu_name()}), flush=True)
+    cases = [('f32', (64, 4, 1 << 20), 1024, 0.64e-6, 641.9, 1300.78125, 1.5625, True),
+             ('u8', (4096, 131072), 256, 64e-6, 1.4, 1500.0, -300.0 / 4096, False),
+             ('u8', (4096, 131072), 256, 64e-6, 300.0, 1500.0, -300.0 / 4096, False)]
+    for dt, shape, nbin, tsamp, nu, f0, df, coherent in cases:
+        nchan, ntime = shape[0], shape[-1]
+        rows = int(np.prod(shape[:-1]))
+        freqs = f0 + df * np.arange(nchan) + (0.5 * abs(df) if coherent else 0.0)
+        delays = bf.fold.dispersion_delays(freqs, 100.0, freqs.max())
+        g = torch.Generator(device='cuda').manual_seed(2)
+        if dt == 'u8':
+            xt = torch.randint(0, 256, shape, dtype=torch.uint8, device='cuda', generator=g)
+        else:
+            xt = torch.rand(shape, dtype=torch.float32, device='cuda', generator=g) * 100
+        d_x = bf.empty(shape, dt, 'cuda')
+        nbytes = xt.numel() * xt.element_size()
+        _check(_bf.bfMemcpy(d_x.ctypes.data, _bf.BF_SPACE_CUDA, xt.data_ptr(), _bf.BF_SPACE_CUDA, nbytes))
+        plan = bf.fold.Fold()
+        plan.init(nbin, delays, tsamp, 0.0, nu)
+        d_o = bf.empty(shape[:-1] + (nbin,), 'f32', 'cuda')
+        d_n = bf.empty((nchan, nbin), 'i32', 'cuda')
+        a_t = torch.from_numpy(0.0 - delays).cuda()
+        t_out = {}
+
+        def torch_fold():
+            t = torch.arange(ntime, dtype=torch.int64, device='cuda').double()
+            tau = a_t[:, None] + t[None, :] * tsamp
+            phi = tau * nu
+            frac = phi - torch.floor(phi)
+            b = torch.clamp(torch.floor(frac * nbin).long(), max=nbin - 1)          # [nchan, ntime]
+            idx = b.reshape((nchan,) + (1,) * (len(shape) - 2) + (ntime,)).expand(shape).reshape(rows, ntime)
+            out = torch.zeros(rows, nbin, dtype=torch.float32, device='cuda')
+            out.scatter_add_(1, idx, xt.reshape(rows, ntime).float())
+            cnt = torch.zeros(nchan, nbin, dtype=torch.int64, device='cuda')
+            cnt.scatter_add_(1, b, torch.ones_like(b))
+            t_out['out'], t_out['cnt'] = out, cnt
+        dst = torch.empty_like(xt)
+        fns = {'new': lambda: plan.execute(d_x, d_o, d_n), 'torch': torch_fold, 'copy': lambda: dst.copy_(xt)}
+        for _ in range(3):
+            for fn in fns.values():
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in fns}
+        for _ in range(nrep):
+            for key, fn in fns.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1))
+        ms = {key: float(np.median(v)) for key, v in times.items()}
+        o1 = np.asarray(d_o.copy('system')).reshape(rows, nbin)
+        n1 = np.asarray(d_n.copy('system'))
+        plan.execute(d_x, d_o, d_n)
+        bf.device.stream_synchronize()
+        identical = bool(np.array_equal(o1.view(np.uint32), np.asarray(d_o.copy('system')).reshape(rows, nbin)
+                                        .view(np.uint32)))
+        to = t_out['out'].cpu().numpy()
+        counts_match = bool(np.array_equal(n1, t_out['cnt'].cpu().numpy()))
+        rel = float(np.max(np.abs(o1.astype(np.float64) - to) / np.maximum(np.abs(to), 1e-30)))
+        nsamp = rows * ntime
+        hbm_ms = nbytes / 3.35e12 * 1e3
+        fp64_ms = nsamp * FOLD_FP64_OPS / FOLD_FP64_RATE * 1e3
+        report('fold %s %s nbin=%d nu=%g tsamp=%g' % (dt, 'x'.join(map(str, shape)), nbin, nu, tsamp), ms['new'],
+               nbytes, samples_per_bin_turn=round(1.0 / (nu * tsamp) / nbin, 3),
+               hbm_bound_ms=round(hbm_ms, 4), fp64_bound_ms=round(fp64_ms, 4),
+               bound='fp64' if fp64_ms > hbm_ms else 'HBM',
+               share_of_bound=round(max(hbm_ms, fp64_ms) / ms['new'], 3),
+               torch_ms=round(ms['torch'], 4), copy_ms=round(ms['copy'], 4),
+               speedup_vs_torch=round(ms['torch'] / ms['new'], 2),
+               counts_match_torch=counts_match, max_rel_vs_torch=rel, identical=identical)
+        del d_x, d_o, d_n, xt, dst, t_out, plan
         torch.cuda.empty_cache()
 
 
