@@ -4,7 +4,6 @@ import math
 
 from bifrost_b200.pipeline import TransformBlock
 from bifrost_b200.coherent_dedisp import CoherentDedisp, dispersion_overlap, default_nfft
-from bifrost_b200.units import convert_units
 from bifrost_b200.blocks import _header as H
 
 CD_DTYPES = ('ci4', 'ci8', 'ci16', 'cf32')
@@ -14,20 +13,11 @@ DM_UNITS = 'pc cm^-3'
 def _band(ihdr):
     """(tensor, nchan, f0 MHz, df MHz) of a ['freq', ..., 'time'] voltage
     header; refuses anything the operation does not take."""
-    t = ihdr['_tensor']
-    labels = list(t.get('labels') or [])
-    if len(labels) < 2 or labels[0] != 'freq' or labels[-1] != 'time' or t['shape'][-1] != -1:
-        raise KeyError("Expected axes ['freq', ..., 'time'] with time as the frame axis, got %s" % labels)
-    if t['dtype'] not in CD_DTYPES:
-        raise TypeError("coherent_dedisp takes %s voltages, got %s" % ('/'.join(CD_DTYPES), t['dtype']))
-    funit, tunit = t['units'][0], t['units'][-1]
-    f0 = convert_units(t['scales'][0][0], funit, 'MHz')
-    df = convert_units(t['scales'][0][1], funit, 'MHz')
-    tsamp = convert_units(t['scales'][-1][1], tunit, 's')
+    t, nchan, f0, df, tsamp = H.channel_band(ihdr, CD_DTYPES, 'coherent_dedisp', 'voltages')
     if df == 0 or abs(abs(tsamp) * abs(df) * 1e6 - 1.0) > 1e-6:
         raise ValueError("coherent_dedisp needs critically sampled channels: |time step| (%g s) must be "
                          "1/|channel width| (%g MHz)" % (tsamp, df))
-    return t, t['shape'][0], f0, df
+    return t, nchan, f0, df
 
 
 def coherent_dedisp_header(ihdr, dm, nfft=None):

@@ -14,24 +14,6 @@ MJD_UNIX_EPOCH = 40587
 COUNT_MAX = 1 << 31
 
 
-def _axes(ihdr):
-    """(tensor, nchan, f0 MHz, df MHz, tsamp s) of a ['freq', ..., 'time']
-    power header; refuses anything the operation does not take."""
-    t = ihdr['_tensor']
-    labels = list(t.get('labels') or [])
-    if len(labels) < 2 or labels[0] != 'freq' or labels[-1] != 'time' or t['shape'][-1] != -1:
-        raise KeyError("Expected axes ['freq', ..., 'time'] with time as the frame axis, got %s" % labels)
-    if t['dtype'] not in FOLD_DTYPES:
-        raise TypeError("fold takes %s power, got %s" % ('/'.join(FOLD_DTYPES), t['dtype']))
-    funit, tunit = t['units'][0], t['units'][-1]
-    f0 = convert_units(t['scales'][0][0], funit, 'MHz')
-    df = convert_units(t['scales'][0][1], funit, 'MHz')
-    tsamp = abs(convert_units(t['scales'][-1][1], tunit, 's'))
-    if tsamp == 0:
-        raise ValueError("the time axis has no sampling step")
-    return t, t['shape'][0], f0, df, tsamp
-
-
 def fold_header(ihdr, nbin, nu, nudot=0., nuddot=0., pepoch=None, dm=None, tsubint=None, gulp_nframe=None):
     """(output header, delays s, tsamp s, t0 s, nsamp_sub) of fold(nbin, nu,
     nudot, nuddot, pepoch, dm, tsubint) on a ['freq', ..., 'time'] u8 / u16 /
@@ -46,7 +28,10 @@ def fold_header(ihdr, nbin, nu, nudot=0., nuddot=0., pepoch=None, dm=None, tsubi
     s) - (pepoch - 40587) 86400.  A subintegration is tsubint s rounded to
     whole samples, which must be a positive multiple of the gulp (None: one
     gulp)."""
-    t, nchan, f0, df, tsamp = _axes(ihdr)
+    t, nchan, f0, df, tsamp = H.channel_band(ihdr, FOLD_DTYPES, 'fold', 'power')
+    tsamp = abs(tsamp)
+    if tsamp == 0:
+        raise ValueError("the time axis has no sampling step")
     if dm is None:
         if 'coherent_dm' not in ihdr:
             raise ValueError("fold needs dm= when the input was not coherently dedispersed")

@@ -13,10 +13,7 @@ def pulse_search_header(ihdr, widths, decim):
     f32 sequence with header ihdr: the time axis (still the frame axis) steps
     by decim samples and a last 'peak' axis of length 3 holds PEAK_FIELDS."""
     ohdr, t = H.derive(ihdr)
-    if t['shape'][-1] != -1 or t.get('labels', [None])[-1] != 'time':
-        raise KeyError("Expected axes [..., 'time'] with time as the frame axis, got %s" % t.get('labels'))
-    if t['dtype'] != 'f32':
-        raise TypeError("pulse_search takes f32 input, got %s" % t['dtype'])
+    H.check_time_frames(t, ('f32',), 'pulse_search', 'input')
     H.scale_step(t, len(t['shape']) - 1, decim)
     for key, value in (('shape', 3), ('labels', 'peak'), ('scales', None), ('units', None)):
         if key in t:

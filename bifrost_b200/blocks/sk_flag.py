@@ -12,10 +12,7 @@ def sk_flag_header(ihdr, window, nacc=1, shape=1.0, sigma=3.0):
     [..., 'time'] u8 / u16 / f32 sequence with header ihdr: the input's,
     plus sk_window, sk_nacc, sk_shape and sk_thresholds = [lo, hi]."""
     ohdr, t = H.derive(ihdr)
-    if t['shape'][-1] != -1 or t.get('labels', [None])[-1] != 'time':
-        raise KeyError("Expected axes [..., 'time'] with time as the frame axis, got %s" % t.get('labels'))
-    if t['dtype'] not in SK_DTYPES:
-        raise TypeError("sk_flag takes %s power, got %s" % ('/'.join(SK_DTYPES), t['dtype']))
+    H.check_time_frames(t, SK_DTYPES, 'sk_flag', 'power')
     ohdr.update(sk_window=int(window), sk_nacc=int(nacc), sk_shape=float(shape),
                 sk_thresholds=list(sk_thresholds(window, nacc, shape, sigma)))
     return ohdr

@@ -7,10 +7,9 @@ filtered by overlap-save with N-point segments and the inverse of the
 cold-plasma transfer function, which aligns every output sample to the
 arrival time at its channel's top edge.  Output t depends on the input from
 t to t + overlap.  The output is cf32; integer inputs enter unscaled."""
-import ctypes
 import math
 
-from bifrost_b200.libbifrost import _bf, _check, _get, BifrostObject
+from bifrost_b200.libbifrost import _bf, _check, _exec_storage, _get, BifrostObject
 from bifrost_b200.ndarray import asarray
 
 KDM = 4.148741601e3          # MHz^2 pc^-1 cm^3 s
@@ -54,18 +53,18 @@ class CoherentDedisp(BifrostObject):
         self.nchan, self.f0, self.df, self.dm, self.nfft = int(nchan), float(f0), float(df), float(dm), int(nfft)
         self.overlap = int(_get(_bf.bfCoherentDedispGetOverlap, self.obj))
 
+    def _run(self, idata, odata, **storage):
+        return _exec_storage(_bf.bfCoherentDedispExecute, self.obj, asarray(idata).as_BFarray(),
+                             asarray(odata).as_BFarray(), **storage)
+
     def execute(self, idata, odata):
         """odata (cf32, idata's shape) = idata dedispersed."""
-        _check(_bf.bfCoherentDedispExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
-                                           None, None))
+        self._run(idata, odata)
         return odata
 
     def get_workspace_size(self, idata, odata):
-        return _get(_bf.bfCoherentDedispExecute, self.obj, asarray(idata).as_BFarray(),
-                    asarray(odata).as_BFarray(), None)
+        return self._run(idata, odata, query=True)
 
     def execute_workspace(self, idata, odata, workspace_ptr, workspace_size):
-        size = _bf.BFsize(workspace_size)
-        _check(_bf.bfCoherentDedispExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
-                                           workspace_ptr, ctypes.byref(size)))
+        self._run(idata, odata, workspace=(workspace_ptr, workspace_size))
         return odata

@@ -25,7 +25,7 @@
 //       coherent_dedisp_keep_kernel (the kept L samples of each segment).
 //
 // Both paths take phi_k from cd_chirp.  No atomics: two runs give the same bits.
-#include "core.hpp"
+#include "shape.hpp"
 #include "fft4096.cuh"
 
 #include <algorithm>
@@ -42,12 +42,9 @@ constexpr int    CD_NFUSE = 4096;             // longest transform of the fused 
 enum CdKind { CD_CF32 = 0, CD_CI8, CD_CI16, CD_CI4 };
 
 struct CdParams {
-	const char* in;               // bytes
-	float2*     out;              // cf32
-	int  nrowdim;                 // dims before time (axis 0 = channel)
-	long rshape[BF_MAX_DIMS];
-	long istride[BF_MAX_DIMS];    // bytes
-	long ostride[BF_MAX_DIMS];    // float2 elements
+	const char* in;
+	char*       out;              // cf32
+	RowBatch<long, 2> rows;       // in, out: dims before time (axis 0 = channel)
 	long ntime;
 	int  N, L;
 	long nseg;                    // segments per row
@@ -79,17 +76,6 @@ __device__ __forceinline__ float2 cd_load(const char* row, long t) {
 	if( KIND == CD_CI16 ) { const short2 v = ((const short2*)row)[t]; return make_float2(v.x, v.y); }
 	const signed char b = ((const signed char*)row)[t];          // high nibble real, low nibble imaginary
 	return make_float2((float)((signed char)(b & 0xF0) >> 4), (float)((signed char)(b << 4) >> 4));
-}
-
-__device__ __forceinline__ void cd_row_offsets(CdParams const& P, long r, long* io, long* oo) {
-	long a = 0, b = 0;
-	for( int d=P.nrowdim-1; d>=0; --d ) {
-		const long i = r % P.rshape[d];
-		r /= P.rshape[d];
-		a += i * P.istride[d];
-		b += i * P.ostride[d];
-	}
-	*io = a; *oo = b;
 }
 
 // --------------------------------------------------------------- fused path
@@ -180,9 +166,9 @@ coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
 		const bool live = line < nline;
 		const long b = live ? line / P.nseg : 0;
 		const long t0 = live ? (line - b * P.nseg) * P.L : 0;
-		long io, oo;
-		cd_row_offsets(P, c * P.nbatch + b, &io, &oo);
-		const char* irow = P.in + io;
+		long off[2];
+		P.rows.offsets(c * P.nbatch + b, off);
+		const char* irow = P.in + off[0];
 		float vr[16], vi[16];
 #pragma unroll
 		for( int m=0; m<16; ++m ) {
@@ -205,7 +191,7 @@ coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
 		for( int m=0; m<16; ++m ) { const float2 v = buf[spad(p + T * m)]; vr[m] = v.x; vi[m] = v.y; }
 		cd_fft<R3>(vr, vi, buf, tb, tid, p);
 		if( live ) {
-			float2* orow = P.out + oo;
+			float2* orow = (float2*)(P.out + off[1]);
 			const long keep = min((long)P.L, P.ntime - t0);
 #pragma unroll
 			for( int s=0; s<16; ++s ) {
@@ -228,9 +214,9 @@ coherent_dedisp_gather_kernel(const __grid_constant__ CdParams P, long nrows) {
 		const long t = s * P.L + e;
 		float2 v = make_float2(0.f, 0.f);
 		if( t < P.ntime ) {
-			long io, oo;
-			cd_row_offsets(P, r, &io, &oo);
-			v = cd_load<KIND>(P.in + io, t);
+			long off[2];
+			P.rows.offsets(r, off);
+			v = cd_load<KIND>(P.in + off[0], t);
 		}
 		P.ws[i] = v;
 	}
@@ -254,9 +240,9 @@ coherent_dedisp_keep_kernel(const __grid_constant__ CdParams P, long nrows) {
 	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
 		const long r = i / P.ntime, t = i - r * P.ntime;
 		const long s = t / P.L, e = t - s * P.L;
-		long io, oo;
-		cd_row_offsets(P, r, &io, &oo);
-		P.out[oo + t] = P.ws[(r * P.nseg + s) * P.N + e];
+		long off[2];
+		P.rows.offsets(r, off);
+		((float2*)(P.out + off[1]))[t] = P.ws[(r * P.nseg + s) * P.N + e];
 	}
 }
 
@@ -271,12 +257,8 @@ struct BFcoherentdedisp_impl {
 	BFfft  fft = nullptr;         // long path: one plan over [rows * nseg, N], run both ways
 	long   fft_lines = -1;
 	size_t fft_tmp = 0;
-	void*  own_ws = nullptr;
-	size_t own_size = 0;
-	~BFcoherentdedisp_impl() {
-		if( fft ) bfFftDestroy(fft);
-		if( own_ws ) cudaFree(own_ws);
-	}
+	DeviceBuffer ws;
+	~BFcoherentdedisp_impl() { if( fft ) bfFftDestroy(fft); }
 };
 
 namespace {
@@ -361,17 +343,15 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 	const int kind = cd_kind(in->dtype);
 	BFB_ASSERT(kind >= 0 && out->dtype == BF_DTYPE_CF32, BF_STATUS_UNSUPPORTED_DTYPE);
 	const int nd = in->ndim;
-	BFB_ASSERT(nd >= 2 && nd <= BF_MAX_DIMS && out->ndim == nd, BF_STATUS_INVALID_SHAPE);
-	for( int d=0; d<nd; ++d ) BFB_ASSERT(in->shape[d] == out->shape[d], BF_STATUS_INVALID_SHAPE);
+	BFarray const* const ops[2] = {in, out};
+	BFB_ASSERT(nd >= 2 && rows_match(ops, nd - 1, {1, 1}), BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(out->shape[nd-1] == in->shape[nd-1], BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(in->shape[0] == plan->nchan, BF_STATUS_INVALID_SHAPE);
-	const long isz = dtype_nbyte(in->dtype);
-	BFB_ASSERT(in->strides[nd-1] == isz && out->strides[nd-1] == 8, BF_STATUS_UNSUPPORTED_STRIDE);
-	BFB_ASSERT((uintptr_t)in->data % isz == 0 && (uintptr_t)out->data % 8 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd-1; ++d )
-		BFB_ASSERT(in->strides[d] % isz == 0 && out->strides[d] % 8 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	CdParams P = {};
+	long nrows;
+	BFstatus s = row_batch(ops, nd - 1, &P.rows, &nrows);
+	if( s != BF_STATUS_SUCCESS ) return s;
 	const long ntime = in->shape[nd-1];
-	long nrows = 1;
-	for( int d=0; d<nd-1; ++d ) nrows *= in->shape[d];
 	const long nchan = plan->nchan;
 	BFB_ASSERT(nchan <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);      // channels run on gridDim.y
 	const long N = plan->nfft, L = N - plan->overlap;
@@ -381,35 +361,17 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 	size_t need = 0, seg_bytes = 0;
 	if( !fused && nrows * nseg > 0 ) {
 		seg_bytes = round_up<size_t>((size_t)(nrows * nseg * N) * 8, CD_ALIGN);
-		BFstatus s = cd_plan_fft(plan, nrows * nseg);
+		s = cd_plan_fft(plan, nrows * nseg);
 		if( s != BF_STATUS_SUCCESS ) return s;
 		need = seg_bytes + round_up<size_t>(plan->fft_tmp, CD_ALIGN);
 	}
-	need = std::max(need, CD_ALIGN);
-	if( exec_storage_size ) {
-		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_size < need ) {
-			if( plan->own_ws ) cudaFree(plan->own_ws);
-			plan->own_ws = nullptr; plan->own_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_ws, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_size = need;
-		}
-		exec_storage = plan->own_ws;
-	}
+	void* mem;
+	s = use_storage(plan->ws, std::max(need, CD_ALIGN), exec_storage, exec_storage_size, &mem);
+	if( s != BF_STATUS_SUCCESS || !mem ) return s;
 	if( nrows == 0 || ntime == 0 ) return BF_STATUS_SUCCESS;
 
-	CdParams P = {};
 	P.in  = (const char*)in->data;
-	P.out = (float2*)out->data;
-	P.nrowdim = nd - 1;
-	for( int d=0; d<nd-1; ++d ) {
-		P.rshape[d]  = in->shape[d];
-		P.istride[d] = in->strides[d];
-		P.ostride[d] = out->strides[d] / 8;
-	}
+	P.out = (char*)out->data;
 	P.ntime  = ntime;
 	P.N      = (int)N;
 	P.L      = (int)L;
@@ -429,8 +391,8 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 		BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 		return BF_STATUS_SUCCESS;
 	}
-	P.ws = (float2*)exec_storage;
-	void* tmp = (char*)exec_storage + seg_bytes;
+	P.ws = (float2*)mem;
+	void* tmp = (char*)mem + seg_bytes;
 	const long nws = nrows * nseg * N;
 	switch( kind ) {
 	case CD_CF32: coherent_dedisp_gather_kernel<CD_CF32><<<cd_grid(nws), 256, 0, st>>>(P, nrows); break;
@@ -441,7 +403,7 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 	count_launch();
 	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 	const BFarray seg = cd_seg_array(P.ws, nrows * nseg, N);
-	BFstatus s = bfFftExecute(plan->fft, &seg, &seg, 0, tmp, plan->fft_tmp);
+	s = bfFftExecute(plan->fft, &seg, &seg, 0, tmp, plan->fft_tmp);
 	if( s != BF_STATUS_SUCCESS ) return s;
 	coherent_dedisp_chirp_kernel<<<cd_grid(nws), 256, 0, st>>>(P, nrows);
 	count_launch();
@@ -458,12 +420,7 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 
 extern "C" {
 
-BFstatus bfCoherentDedispCreate(BFcoherentdedisp* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFcoherentdedisp_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfCoherentDedispCreate(BFcoherentdedisp* plan_ptr) { return create_handle(plan_ptr); }
 
 BFstatus bfCoherentDedispInit(BFcoherentdedisp plan, BFsize nchan, double f0, double df,
                               double dm, BFsize nfft) {
@@ -510,10 +467,6 @@ BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarr
 	BFB_TRY(return cd_execute(plan, in, out, exec_storage, exec_storage_size));
 }
 
-BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan) { return destroy_handle(plan); }
 
 } // extern "C"

@@ -1,6 +1,7 @@
 // core.hpp -- internal helpers shared by every translation unit of
 // libbifrost_b200: status plumbing, dtype arithmetic, BFarray shape
-// canonicalisation, the per-thread stream and the launch counter.
+// canonicalisation, the per-thread stream, the launch counter, and plan
+// handles and their device storage.
 #pragma once
 
 #include <bifrost_b200.h>
@@ -99,6 +100,63 @@ inline unsigned long pow2_alignment(unsigned long x, unsigned long cap) {
 	unsigned long a = cap;
 	while( a > 1 && (x % a) != 0 ) a >>= 1;
 	return a;
+}
+
+// ---- plan handles and storage ----------------------------------------------
+// bf*Create / bf*Destroy of a plan handle T*.
+template<typename T> BFstatus create_handle(T** plan_ptr) {
+	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
+	*plan_ptr = nullptr;
+	BFB_TRY(*plan_ptr = new T());
+	return BF_STATUS_SUCCESS;
+}
+
+template<typename T> BFstatus destroy_handle(T* plan) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	delete plan;
+	return BF_STATUS_SUCCESS;
+}
+
+// Device memory owned by a plan.  It only grows: a larger request frees the
+// old block before allocating, and a failed allocation leaves it empty.
+class DeviceBuffer {
+	void*  ptr_  = nullptr;
+	size_t size_ = 0;
+public:
+	DeviceBuffer() = default;
+	DeviceBuffer(DeviceBuffer const&) = delete;
+	DeviceBuffer& operator=(DeviceBuffer const&) = delete;
+	~DeviceBuffer() { if( ptr_ ) cudaFree(ptr_); }
+	void* data() const { return ptr_; }
+	cudaError_t reserve(size_t size) {
+		if( size_ >= size ) return cudaSuccess;
+		if( ptr_ ) cudaFree(ptr_);
+		ptr_ = nullptr; size_ = 0;
+		const cudaError_t e = cudaMalloc(&ptr_, size);
+		if( e == cudaSuccess ) size_ = size;
+		else ptr_ = nullptr;
+		return e;
+	}
+};
+
+// The plan_storage / exec_storage protocol (include/bifrost_b200.h, FDMT):
+// (NULL, &size) stores the `need` bytes in *size, a query only; (ptr, &size)
+// runs in the caller's ptr, which must hold `need` bytes; (NULL, NULL) runs
+// in `own`, grown to `need`; (ptr, NULL) is refused.  On success *use is the
+// memory to run in, or NULL after a query (need > 0, so never otherwise).
+inline BFstatus use_storage(DeviceBuffer& own, size_t need, void* storage, BFsize* storage_size,
+                            void** use) {
+	*use = nullptr;
+	if( storage_size ) {
+		if( !storage ) { *storage_size = need; return BF_STATUS_SUCCESS; }
+		BFB_ASSERT(*storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
+		*use = storage;
+	} else {
+		BFB_ASSERT(!storage, BF_STATUS_INVALID_ARGUMENT);
+		BFB_CUDA(own.reserve(need), BF_STATUS_MEM_ALLOC_FAILED);
+		*use = own.data();
+	}
+	return BF_STATUS_SUCCESS;
 }
 
 } // namespace bfb

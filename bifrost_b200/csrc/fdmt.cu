@@ -470,8 +470,7 @@ struct BFfdmt_impl {
 	cudaStream_t stream = nullptr;
 	bool     stream_set = false;
 	// device plan
-	void*  own_plan_storage = nullptr;
-	size_t own_plan_size = 0;
+	DeviceBuffer own_plan;
 	int*   d_row_offsets = nullptr;      // [nchan+1]
 	int4*  d_rows = nullptr;             // [nstep][plan_stride]
 	int2*  d_row0map = nullptr;          // [nrow(0)]
@@ -514,8 +513,7 @@ struct BFfdmt_impl {
 	std::vector<std::vector<int> > shard_progs;
 	std::vector<int*> d_shard_progs;
 	// exec workspace
-	void*  own_exec_storage = nullptr;
-	size_t own_exec_size = 0;
+	DeviceBuffer own_exec;
 
 	cudaStream_t get_stream() { return stream_set ? stream : thread_stream(); }
 
@@ -526,8 +524,6 @@ struct BFfdmt_impl {
 		return off_head() + round_up<size_t>(plan.bands[K].size() * sizeof(HeadBand), 512);
 	}
 	~BFfdmt_impl() {
-		if( own_plan_storage ) cudaFree(own_plan_storage);
-		if( own_exec_storage ) cudaFree(own_exec_storage);
 		if( d_items ) cudaFree(d_items);
 		free_passes();
 	}
@@ -1120,18 +1116,9 @@ static size_t mega_geometry(std::vector<PackedPass> const& cps, long C, int lag,
 }
 extern "C" {
 
-BFstatus bfFdmtCreate(BFfdmt* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFfdmt_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFdmtCreate(BFfdmt* plan_ptr) { return create_handle(plan_ptr); }
 
-BFstatus bfFdmtDestroy(BFfdmt plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFdmtDestroy(BFfdmt plan) { return destroy_handle(plan); }
 
 BFstatus bfFdmtSetStream(BFfdmt plan, void const* stream) {
 	BFB_ASSERT(plan,   BF_STATUS_INVALID_HANDLE);
@@ -1170,21 +1157,10 @@ BFstatus bfFdmtInit(BFfdmt plan, BFsize nchan, BFsize max_delay,
 	for( int s=1; s<P.nstep(); ++s ) {
 		for( FdmtRow const& r : P.rows[s] ) plan->step_maxdelay[s] = std::max(plan->step_maxdelay[s], r.delay);
 	}
-	size_t need = plan->plan_bytes();
-	if( plan_storage_size ) {
-		if( !plan_storage ) { *plan_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*plan_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!plan_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_plan_size < need ) {
-			if( plan->own_plan_storage ) cudaFree(plan->own_plan_storage);
-			plan->own_plan_storage = nullptr; plan->own_plan_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_plan_storage, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_plan_size = need;
-		}
-		plan_storage = plan->own_plan_storage;
-	}
-	char* base = (char*)plan_storage;
+	void* mem;
+	const BFstatus status = use_storage(plan->own_plan, plan->plan_bytes(), plan_storage, plan_storage_size, &mem);
+	if( status != BF_STATUS_SUCCESS || !mem ) return status;
+	char* base = (char*)mem;
 	plan->d_row_offsets = (int*)base;
 	plan->d_rows    = (int4*)(base + plan->off_rows());
 	plan->d_row0map = (int2*)(base + plan->off_row0map());
@@ -1669,19 +1645,8 @@ BFstatus bfFdmtExecute(BFfdmt plan, BFarray const* in, BFarray const* out,
 			need = chunks.bytes;
 		}
 	}
-	if( exec_storage_size ) {
-		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_exec_size < need ) {
-			if( plan->own_exec_storage ) cudaFree(plan->own_exec_storage);
-			plan->own_exec_storage = nullptr; plan->own_exec_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_exec_storage, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_exec_size = need;
-		}
-		exec_storage = plan->own_exec_storage;
-	}
+	const BFstatus status = use_storage(plan->own_exec, need, exec_storage, exec_storage_size, &exec_storage);
+	if( status != BF_STATUS_SUCCESS || !exec_storage ) return status;
 	BFB_ASSERT(space_on_device(in->space),  BF_STATUS_UNSUPPORTED_SPACE);
 	BFB_ASSERT(space_on_device(out->space), BF_STATUS_UNSUPPORTED_SPACE);
 	BFB_ASSERT(out->dtype == BF_DTYPE_F32,  BF_STATUS_UNSUPPORTED_DTYPE);

@@ -643,8 +643,7 @@ struct BFfft_impl {
 	std::map<long, void*> twid;          // n -> table of n pairs
 	std::map<long, void*> tw_lo, tw_hi;  // four-step N -> tables
 	std::map<long, void*> chirp, chirp_spec;   // Bluestein: n -> exp(-i pi j^2 / n) and the spectrum of its conjugate, length m
-	void*  own_ws = nullptr;
-	size_t own_ws_size = 0;
+	DeviceBuffer ws;                  // library-managed tmp_storage
 	bool   planned = false;
 
 	~BFfft_impl() {
@@ -653,7 +652,6 @@ struct BFfft_impl {
 		for( auto& kv : tw_hi ) cudaFree(kv.second);
 		for( auto& kv : chirp ) cudaFree(kv.second);
 		for( auto& kv : chirp_spec ) cudaFree(kv.second);
-		if( own_ws ) cudaFree(own_ws);
 	}
 };
 
@@ -1250,18 +1248,9 @@ BFstatus run_axis(BFfft_impl* plan, int ndim, const long* batch_shape, int axis,
 
 extern "C" {
 
-BFstatus bfFftCreate(BFfft* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFfft_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFftCreate(BFfft* plan_ptr) { return create_handle(plan_ptr); }
 
-BFstatus bfFftDestroy(BFfft plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFftDestroy(BFfft plan) { return destroy_handle(plan); }
 
 BFstatus bfFftInit(BFfft plan, BFarray const* in, BFarray const* out, int rank,
                    int const* axes, BFbool apply_fftshift, size_t* tmp_storage_size) {
@@ -1364,13 +1353,8 @@ BFstatus bfFftExecute(BFfft plan, BFarray const* in, BFarray const* out, BFbool 
 	cudaStream_t st = thread_stream();
 	if( plan->workspace_size ) {
 		if( !tmp_storage ) {
-			if( plan->own_ws_size < plan->workspace_size ) {
-				if( plan->own_ws ) cudaFree(plan->own_ws);
-				plan->own_ws = nullptr; plan->own_ws_size = 0;
-				BFB_CUDA(cudaMalloc(&plan->own_ws, plan->workspace_size), BF_STATUS_MEM_ALLOC_FAILED);
-				plan->own_ws_size = plan->workspace_size;
-			}
-			tmp_storage = plan->own_ws;
+			BFB_CUDA(plan->ws.reserve(plan->workspace_size), BF_STATUS_MEM_ALLOC_FAILED);
+			tmp_storage = plan->ws.data();
 		} else {
 			BFB_ASSERT(tmp_storage_size >= plan->workspace_size, BF_STATUS_INSUFFICIENT_STORAGE);
 		}

@@ -30,7 +30,7 @@
 //
 // No atomics: two runs on the same input give the same bits.  Limits: nbin
 // <= 4096, rows and ntime within 32 bits, counts below 2^31.
-#include "core.hpp"
+#include "shape.hpp"
 
 #include <algorithm>
 #include <climits>
@@ -44,11 +44,8 @@ constexpr int FOLD_FIN_THREADS = 256;
 constexpr long FOLD_TARGET_CTAS = 132L * 32 * 4;      // about four waves of one-warp CTAs on 132 SMs
 
 struct FoldParams {
-	const char* in;               // x, bytes
-	int  nrowdim;                 // leading dims of x (channel first)
-	int  rshape[BF_MAX_DIMS];
-	long xstride[BF_MAX_DIMS];    // bytes
-	long ostride[BF_MAX_DIMS];    // out, floats
+	const char* in;               // x
+	RowBatch<int, 2> rows;        // x, out: leading dims of x (channel first)
 	long cstride;                 // count channel stride, ints
 	int  ntime, nbin, nslice, cps;   // cps: 16-byte chunks per slice (a multiple of 32)
 	int  nrows, nchan, rpc;       // rpc: rows per channel
@@ -57,20 +54,10 @@ struct FoldParams {
 	const double* a;              // [nchan]: t0 - delay[c]
 	double* prof;                 // [row][slice][bin]
 	int*    cnt;                  // [chan][slice][bin]
-	float*  out;
+	char*   out;
 	int*    count;
 	int     accumulate;
 };
-
-__device__ __forceinline__ long fold_row_offset(FoldParams const& P, int r, const long* stride) {
-	long o = 0;
-	for( int d=P.nrowdim-1; d>=0; --d ) {
-		int i = r % P.rshape[d];
-		r /= P.rshape[d];
-		o += i * stride[d];
-	}
-	return o;
-}
 
 // The bin of sample t of a row whose channel has a = t0 - delay[c].
 __device__ __forceinline__ int fold_bin(FoldParams const& P, double a, long long t) {
@@ -131,7 +118,9 @@ fold_kernel(const __grid_constant__ FoldParams P) {
 	const bool first_row = row % P.rpc == 0;
 	for( int b=lane; b<P.nbin; b+=32 ) { prof[b] = 0.; cnt[b] = 0; }
 
-	const T* x = (const T*)(P.in + fold_row_offset(P, row, P.xstride));
+	long off[2];
+	P.rows.offsets(row, off);
+	const T* x = (const T*)(P.in + off[0]);
 	// chunk k of the row covers samples [k E - mis, k E - mis + E)
 	const int mis = (int)(((uintptr_t)x & 15) / sizeof(T));
 	const uint4* xv = (const uint4*)(x - mis);
@@ -221,7 +210,9 @@ fold_finish_kernel(const __grid_constant__ FoldParams P) {
 		const double* p = P.prof + (size_t)row * P.nslice * P.nbin + b;
 		double s = 0.;
 		for( int k=0; k<P.nslice; ++k ) s = __dadd_rn(s, p[(size_t)k * P.nbin]);
-		float* o = P.out + fold_row_offset(P, row, P.ostride) + b;
+		long off[2];
+		P.rows.offsets(row, off);
+		float* o = (float*)(P.out + off[1]) + b;
 		*o = __double2float_rn(P.accumulate ? __dadd_rn((double)*o, s) : s);
 	} else if( i < nprof + (long)P.nchan * P.nbin ) {
 		const long j = i - nprof;
@@ -245,9 +236,7 @@ struct BFfold_impl {
 	long   nchan = 0;
 	double tsamp = 0., nu = 0., c2 = 0., c3 = 0.;
 	std::vector<double> a;        // t0 - delay[c]
-	void*  own_ws = nullptr;
-	size_t own_size = 0;
-	~BFfold_impl() { if( own_ws ) cudaFree(own_ws); }
+	DeviceBuffer ws;
 };
 
 namespace {
@@ -275,26 +264,24 @@ BFstatus fold_execute(BFfold plan, BFarray const* in, BFoffset first, BFarray co
 	BFB_ASSERT(fold_dtype_ok(in->dtype) && out->dtype == BF_DTYPE_F32 && count->dtype == BF_DTYPE_I32,
 	           BF_STATUS_UNSUPPORTED_DTYPE);
 	const int nd = in->ndim;
-	BFB_ASSERT(nd >= 2 && nd <= BF_MAX_DIMS && out->ndim == nd && count->ndim == 2, BF_STATUS_INVALID_SHAPE);
+	BFarray const* const ops[2] = {in, out};
+	BFB_ASSERT(nd >= 2 && rows_match(ops, nd - 1, {1, 1}) && count->ndim == 2, BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(in->shape[0] == plan->nchan, BF_STATUS_INVALID_SHAPE);
-	for( int d=0; d<nd-1; ++d ) BFB_ASSERT(out->shape[d] == in->shape[d], BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(out->shape[nd-1] == plan->nbin, BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(count->shape[0] == plan->nchan && count->shape[1] == plan->nbin, BF_STATUS_INVALID_SHAPE);
-	const long isz = dtype_nbyte(in->dtype);
-	BFB_ASSERT(in->strides[nd-1] == isz && (uintptr_t)in->data % isz == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd-1; ++d ) BFB_ASSERT(in->strides[d] % isz == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	BFB_ASSERT(out->strides[nd-1] == 4 && (uintptr_t)out->data % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd-1; ++d ) BFB_ASSERT(out->strides[d] % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	FoldParams P = {};
+	long nrows;
+	BFstatus s = row_batch(ops, nd - 1, &P.rows, &nrows);
+	if( s != BF_STATUS_SUCCESS ) return s;
 	BFB_ASSERT(count->strides[1] == 4 && count->strides[0] % 4 == 0 && (uintptr_t)count->data % 4 == 0,
 	           BF_STATUS_UNSUPPORTED_STRIDE);
 	const long ntime = in->shape[nd-1];
-	long nrows = 1;
-	for( int d=0; d<nd-1; ++d ) {
-		BFB_ASSERT(in->shape[d] <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
-		nrows *= in->shape[d];
-		BFB_ASSERT(nrows <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
-	}
 	// rows and sample indices are 32-bit in the kernels (with a chunk of slack)
+	for( long d=0, n=1; d<nd-1; ++d ) {
+		BFB_ASSERT(in->shape[d] <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
+		n *= in->shape[d];
+		BFB_ASSERT(n <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
+	}
 	BFB_ASSERT(ntime <= INT_MAX - 64, BF_STATUS_UNSUPPORTED_SHAPE);
 	const long nchan = plan->nchan, nbin = plan->nbin;
 	const long rpc = nrows / nchan;                    // rows per channel (0 for an empty batch axis)
@@ -302,7 +289,7 @@ BFstatus fold_execute(BFfold plan, BFarray const* in, BFoffset first, BFarray co
 	// Slices: whole groups of 32 chunks, at least 32 nbin samples each so the
 	// profile written per slice stays small next to the samples read, and
 	// enough of them for about FOLD_TARGET_CTAS warps in all.
-	const long E = 16 / isz;
+	const long E = 16 / dtype_nbyte(in->dtype);
 	const long nchunk = div_up(ntime + E - 1, E);      // any row's chunks, whatever its alignment
 	const long min_chunks = round_up(div_up(std::max(8192L, 32 * nbin), E), 32L);
 	const long want = nrows ? div_up(FOLD_TARGET_CTAS, nrows) : 1;
@@ -312,30 +299,13 @@ BFstatus fold_execute(BFfold plan, BFarray const* in, BFoffset first, BFarray co
 	const size_t off_prof = round_up<size_t>((size_t)nchan * sizeof(double), FOLD_ALIGN);
 	const size_t off_cnt  = off_prof + round_up<size_t>((size_t)nrows * nslice * nbin * sizeof(double), FOLD_ALIGN);
 	const size_t need     = off_cnt + round_up<size_t>((size_t)nchan * nslice * nbin * sizeof(int), FOLD_ALIGN);
-	if( exec_storage_size ) {
-		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_size < need ) {
-			if( plan->own_ws ) cudaFree(plan->own_ws);
-			plan->own_ws = nullptr; plan->own_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_ws, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_size = need;
-		}
-		exec_storage = plan->own_ws;
-	}
+	void* mem;
+	s = use_storage(plan->ws, need, exec_storage, exec_storage_size, &mem);
+	if( s != BF_STATUS_SUCCESS || !mem ) return s;
 	if( nrows == 0 ) nslice = 0;
 	if( nslice == 0 && accumulate ) return BF_STATUS_SUCCESS;   // adds nothing
 
-	FoldParams P = {};
 	P.in = (const char*)in->data;
-	P.nrowdim = nd - 1;
-	for( int d=0; d<nd-1; ++d ) {
-		P.rshape[d]  = (int)in->shape[d];
-		P.xstride[d] = in->strides[d];
-		P.ostride[d] = out->strides[d] / 4;
-	}
 	P.cstride = count->strides[0] / 4;
 	P.ntime  = (int)ntime;
 	P.nbin   = (int)nbin;
@@ -349,11 +319,11 @@ BFstatus fold_execute(BFfold plan, BFarray const* in, BFoffset first, BFarray co
 	P.nu     = plan->nu;
 	P.c2     = plan->c2;
 	P.c3     = plan->c3;
-	char* ws = (char*)exec_storage;
+	char* ws = (char*)mem;
 	P.a      = (const double*)ws;
 	P.prof   = (double*)(ws + off_prof);
 	P.cnt    = (int*)(ws + off_cnt);
-	P.out    = (float*)out->data;
+	P.out    = (char*)out->data;
 	P.count  = (int*)count->data;
 	P.accumulate = accumulate ? 1 : 0;
 
@@ -381,12 +351,7 @@ BFstatus fold_execute(BFfold plan, BFarray const* in, BFoffset first, BFarray co
 
 extern "C" {
 
-BFstatus bfFoldCreate(BFfold* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFfold_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFoldCreate(BFfold* plan_ptr) { return create_handle(plan_ptr); }
 
 BFstatus bfFoldInit(BFfold plan, int nbin, BFsize nchan, double const* delays, double tsamp,
                     double t0, double nu, double nudot, double nuddot) {
@@ -417,10 +382,6 @@ BFstatus bfFoldExecute(BFfold plan, BFarray const* in, BFoffset first, BFarray c
 	BFB_TRY(return fold_execute(plan, in, first, out, count, accumulate, exec_storage, exec_storage_size));
 }
 
-BFstatus bfFoldDestroy(BFfold plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfFoldDestroy(BFfold plan) { return destroy_handle(plan); }
 
 } // extern "C"

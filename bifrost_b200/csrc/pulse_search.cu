@@ -30,7 +30,7 @@
 // Every reduction runs in a fixed order and there are no atomics, so two runs
 // on the same input give the same bits.  Non-finite samples only poison the
 // statistics of their own row.
-#include "core.hpp"
+#include "shape.hpp"
 
 #include <algorithm>
 #include <climits>
@@ -46,13 +46,10 @@ constexpr int PS_MAXW    = 4096;   // widest width
 constexpr int PS_MAXNW   = 32;     // widths per plan
 
 struct PsParams {
-	const char* in;               // x, bytes
-	float*      out;
-	int  nrowdim;                 // leading dims of x (batch..., ndm)
-	int  rshape[BF_MAX_DIMS];
-	long ristride[BF_MAX_DIMS];   // bytes
-	long rostride[BF_MAX_DIMS];   // floats
-	long o_blk;                   // output block stride, floats
+	const char* in;               // x
+	char*       out;
+	RowBatch<int, 2> rows;        // x, out: leading dims (batch..., ndm)
+	long o_blk;                   // output block stride, bytes
 	int  nout, decim, seglen, nseg, nsegtot, ntile;   // 32-bit: no 64-bit divisions
 	int  spt;                     // segments per tile
 	int  nwidth, W;
@@ -61,17 +58,6 @@ struct PsParams {
 	double* segval;               // [row][segment][width]: max b_w
 	int*    segidx;               //                        its first start
 };
-
-__device__ __forceinline__ void ps_row_offsets(PsParams const& P, int r, long* io, long* oo) {
-	long i = 0, o = 0;
-	for( int d=P.nrowdim-1; d>=0; --d ) {
-		int x = r % P.rshape[d];
-		r /= P.rshape[d];
-		i += x * P.ristride[d];
-		o += x * P.rostride[d];
-	}
-	*io = i; *oo = o;
-}
 
 // First start and one-past-last start of segment g.
 __device__ __forceinline__ void ps_segment(PsParams const& P, int g, int* lo, int* hi) {
@@ -128,9 +114,9 @@ pulse_search_scan_kernel(const __grid_constant__ PsParams P) {
 	// layout: prefix sums P[0..L] (fp64), then the samples (f32)
 	double* pre = (double*)ps_smem;
 	float*  xs  = (float*)(pre + ((L + 2) & ~1));
-	long io, oo;
-	ps_row_offsets(P, row, &io, &oo);
-	const float* x = (const float*)(P.in + io) + lo;
+	long off[2];
+	P.rows.offsets(row, off);
+	const float* x = (const float*)(P.in + off[0]) + lo;
 	for( int i=tid; i<L; i+=PS_THREADS ) ps_cp_async4(xs + i, x + i);
 	asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;\n" ::: "memory");
 	__syncthreads();
@@ -225,8 +211,8 @@ pulse_search_finish_kernel(const __grid_constant__ PsParams P) {
 		sig[tid] = sqrt(m.m2 / m.n);
 	}
 	__syncthreads();
-	long io, oo;
-	ps_row_offsets(P, row, &io, &oo);
+	long off[2];
+	P.rows.offsets(row, off);
 	const int nblk = (P.nout + P.decim - 1) / P.decim;
 	for( int j=tid; j<nblk; j+=PS_THREADS ) {
 		const int ga = j * P.nseg, gb = min(ga + P.nseg, P.nsegtot);
@@ -244,7 +230,7 @@ pulse_search_finish_kernel(const __grid_constant__ PsParams P) {
 			const double s = sig[wi] > 0. ? (v - mu[wi]) / sig[wi] : 0.;
 			if( wi == 0 || s > best ) { best = s; bw = wi; bt = t; }
 		}
-		float* o = P.out + oo + (long)j * P.o_blk;
+		float* o = (float*)(P.out + off[1] + (long)j * P.o_blk);
 		o[0] = (float)best;
 		o[1] = (float)(bt - j * P.decim);
 		o[2] = (float)P.widths[bw];
@@ -260,9 +246,7 @@ struct BFpulsesearch_impl {
 	int    nwidth = 0;
 	int    widths[PS_MAXNW] = {};
 	long   decim = 0;
-	void*  own_ws = nullptr;
-	size_t own_size = 0;
-	~BFpulsesearch_impl() { if( own_ws ) cudaFree(own_ws); }
+	DeviceBuffer ws;
 };
 
 namespace {
@@ -303,49 +287,29 @@ BFstatus ps_execute(BFpulsesearch plan, BFarray const* in, BFarray const* out,
 	BFB_ASSERT(space_on_device(in->space) && space_on_device(out->space), BF_STATUS_UNSUPPORTED_SPACE);
 	BFB_ASSERT(in->dtype == BF_DTYPE_F32 && out->dtype == BF_DTYPE_F32, BF_STATUS_UNSUPPORTED_DTYPE);
 	const int nd = in->ndim;
-	BFB_ASSERT(nd >= 2 && nd + 1 <= BF_MAX_DIMS && out->ndim == nd + 1, BF_STATUS_INVALID_SHAPE);
-	for( int d=0; d<nd-1; ++d ) BFB_ASSERT(in->shape[d] == out->shape[d], BF_STATUS_INVALID_SHAPE);
+	BFarray const* const ops[2] = {in, out};
+	BFB_ASSERT(nd >= 2 && rows_match(ops, nd - 1, {1, 2}), BF_STATUS_INVALID_SHAPE);
 	const long ntime = in->shape[nd-1];
 	const long W = plan->widths[plan->nwidth - 1];
 	BFB_ASSERT(out->shape[nd] == 3, BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(ntime >= W, BF_STATUS_INVALID_SHAPE);
 	BFB_ASSERT(out->shape[nd-1] == div_up<long>(ntime - W + 1, plan->decim), BF_STATUS_INVALID_SHAPE);
-	BFB_ASSERT(in->strides[nd-1] == 4, BF_STATUS_UNSUPPORTED_STRIDE);
-	BFB_ASSERT(out->strides[nd] == 4, BF_STATUS_UNSUPPORTED_STRIDE);
-	BFB_ASSERT((uintptr_t)in->data % 4 == 0 && (uintptr_t)out->data % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd; ++d ) BFB_ASSERT(in->strides[d] % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd+1; ++d ) BFB_ASSERT(out->strides[d] % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	long nrows = 1;
-	for( int d=0; d<nd-1; ++d ) nrows *= in->shape[d];
+	PsParams P;
+	long nrows;
+	BFstatus s = row_batch(ops, nd - 1, &P.rows, &nrows);
+	if( s != BF_STATUS_SUCCESS ) return s;
+	BFB_ASSERT(out->strides[nd-1] % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
 	PsGeom G = ps_geometry(plan, nrows, ntime);
-	const size_t need = std::max<size_t>(G.bytes, PS_ALIGN);
-	if( exec_storage_size ) {
-		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_size < need ) {
-			if( plan->own_ws ) cudaFree(plan->own_ws);
-			plan->own_ws = nullptr; plan->own_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_ws, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_size = need;
-		}
-		exec_storage = plan->own_ws;
-	}
+	void* mem;
+	s = use_storage(plan->ws, std::max<size_t>(G.bytes, PS_ALIGN), exec_storage, exec_storage_size, &mem);
+	if( s != BF_STATUS_SUCCESS || !mem ) return s;
 	if( nrows == 0 ) return BF_STATUS_SUCCESS;
 	// rows, starts and segments are 32-bit in the kernels
 	BFB_ASSERT(nrows * G.ntile <= INT_MAX && ntime + plan->decim <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
 
-	PsParams P;
 	P.in  = (const char*)in->data;
-	P.out = (float*)out->data;
-	P.nrowdim = nd - 1;
-	for( int d=0; d<nd-1; ++d ) {
-		P.rshape[d]   = (int)in->shape[d];
-		P.ristride[d] = in->strides[d];
-		P.rostride[d] = out->strides[d] / 4;
-	}
-	P.o_blk   = out->strides[nd-1] / 4;
+	P.out = (char*)out->data;
+	P.o_blk   = out->strides[nd-1];
 	P.nout    = (int)G.nout;
 	P.decim   = (int)plan->decim;
 	P.seglen  = (int)G.seglen;
@@ -356,7 +320,7 @@ BFstatus ps_execute(BFpulsesearch plan, BFarray const* in, BFarray const* out,
 	P.nwidth  = plan->nwidth;
 	P.W       = (int)W;
 	for( int k=0; k<PS_MAXNW; ++k ) P.widths[k] = plan->widths[k];
-	char* ws = (char*)exec_storage;
+	char* ws = (char*)mem;
 	P.stats  = (double*)(ws + G.off_stats);
 	P.segval = (double*)(ws + G.off_val);
 	P.segidx = (int*)(ws + G.off_idx);
@@ -379,12 +343,7 @@ BFstatus ps_execute(BFpulsesearch plan, BFarray const* in, BFarray const* out,
 
 extern "C" {
 
-BFstatus bfPulseSearchCreate(BFpulsesearch* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFpulsesearch_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfPulseSearchCreate(BFpulsesearch* plan_ptr) { return create_handle(plan_ptr); }
 
 BFstatus bfPulseSearchInit(BFpulsesearch plan, int nwidth, int const* widths, int decim) {
 	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
@@ -407,10 +366,6 @@ BFstatus bfPulseSearchExecute(BFpulsesearch plan, BFarray const* in, BFarray con
 	BFB_TRY(return ps_execute(plan, in, out, exec_storage, exec_storage_size));
 }
 
-BFstatus bfPulseSearchDestroy(BFpulsesearch plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfPulseSearchDestroy(BFpulsesearch plan) { return destroy_handle(plan); }
 
 } // extern "C"

@@ -24,7 +24,7 @@
 //       row, single elements otherwise.
 //
 // No atomics: two runs on the same input give the same bits.
-#include "core.hpp"
+#include "shape.hpp"
 
 #include <algorithm>
 #include <climits>
@@ -37,14 +37,10 @@ constexpr int SK_MAXWIN    = 1 << 20;
 constexpr int SK_SEG_BYTES = 65536;     // bytes of a row one apply CTA streams (at most)
 
 struct SkParams {
-	const char* in;               // x, bytes
-	char*       out;              // y, bytes
-	float*      sk;               // may be null
-	int  nrowdim;                 // leading dims of x
-	int  rshape[BF_MAX_DIMS];
-	long xstride[BF_MAX_DIMS];    // bytes
-	long ystride[BF_MAX_DIMS];    // bytes
-	long kstride[BF_MAX_DIMS];    // floats
+	const char* in;               // x
+	char*       out;              // y
+	char*       sk;               // may be null
+	RowBatch<int, 3> rows;        // x, y, sk: leading dims of x
 	int  ntime, M, nwin, nrows;   // 32-bit: checked on the host
 	int  glog;                    // log2 of the lanes per window in the stats kernel
 	int  nseg;                    // apply CTAs per row
@@ -54,18 +50,6 @@ struct SkParams {
 	double*        s1;            // [row][window]
 	unsigned char* flag;          // [row][window]
 };
-
-__device__ __forceinline__ void sk_row_offsets(SkParams const& P, int r, long* xo, long* yo, long* ko) {
-	long a = 0, b = 0, c = 0;
-	for( int d=P.nrowdim-1; d>=0; --d ) {
-		int i = r % P.rshape[d];
-		r /= P.rshape[d];
-		a += i * P.xstride[d];
-		b += i * P.ystride[d];
-		c += i * P.kstride[d];
-	}
-	*xo = a; *yo = b; *ko = c;
-}
 
 // Per-type accumulation.  u8: per-lane u32 sums are exact (a lane adds at most
 // 2^15 + 30 samples of at most 255^2), dp4a adds four bytes per instruction.
@@ -147,11 +131,11 @@ sk_stats_kernel(const __grid_constant__ SkParams P) {
 	const bool live = gid < P.nrows * P.nwin;
 	const int row = live ? gid / P.nwin : 0;
 	const int j   = live ? gid % P.nwin : 0;
-	long xo, yo, ko;
-	sk_row_offsets(P, row, &xo, &yo, &ko);
+	long off[3];
+	P.rows.offsets(row, off);
 	const int t0 = j * P.M;
 	const int m  = live ? min(P.M, P.ntime - t0) : 0;
-	const T* x = (const T*)(P.in + xo) + t0;
+	const T* x = (const T*)(P.in + off[0]) + t0;
 	const int mis = (int)(((uintptr_t)x & 15) / sizeof(T));
 	const int h  = min(m, mis ? E - mis : 0);          // scalar head up to the first 16-byte boundary
 	const int nv = (m - h) / E;
@@ -177,7 +161,7 @@ sk_stats_kernel(const __grid_constant__ SkParams P) {
 	const size_t q = (size_t)row * P.nwin + j;
 	P.s1[q]   = S1;
 	P.flag[q] = flagged;
-	if( P.sk ) P.sk[ko + j] = __double2float_rn(sk);
+	if( P.sk ) ((float*)(P.sk + off[2]))[j] = __double2float_rn(sk);
 }
 
 template<typename T> __device__ __forceinline__ T sk_fill_value(double f);
@@ -235,10 +219,10 @@ sk_apply_kernel(const __grid_constant__ SkParams P) {
 	__syncthreads();
 	const T fill = fill_s;
 
-	long xo, yo, ko;
-	sk_row_offsets(P, row, &xo, &yo, &ko);
-	const T* x = (const T*)(P.in + xo);
-	T*       y = (T*)(P.out + yo);
+	long off[3];
+	P.rows.offsets(row, off);
+	const T* x = (const T*)(P.in + off[0]);
+	T*       y = (T*)(P.out + off[1]);
 	const int M = P.M, ntime = P.ntime;
 	if( ((uintptr_t)x & 15) == ((uintptr_t)y & 15) ) {
 		const int mis = (int)(((uintptr_t)y & 15) / sizeof(T));
@@ -292,9 +276,7 @@ struct BFskflag_impl {
 	bool   planned = false;
 	int    window = 0, nacc = 0;
 	double shape = 0., lo = 0., hi = 0.;
-	void*  own_ws = nullptr;
-	size_t own_size = 0;
-	~BFskflag_impl() { if( own_ws ) cudaFree(own_ws); }
+	DeviceBuffer ws;
 };
 
 namespace {
@@ -323,67 +305,41 @@ BFstatus sk_execute(BFskflag plan, BFarray const* x, BFarray const* y, BFarray c
 	BFB_ASSERT(sk_dtype_ok(x->dtype) && y->dtype == x->dtype, BF_STATUS_UNSUPPORTED_DTYPE);
 	BFB_ASSERT(!sk || sk->dtype == BF_DTYPE_F32, BF_STATUS_UNSUPPORTED_DTYPE);
 	const int nd = x->ndim;
-	BFB_ASSERT(nd >= 1 && nd <= BF_MAX_DIMS && y->ndim == nd, BF_STATUS_INVALID_SHAPE);
-	for( int d=0; d<nd; ++d ) BFB_ASSERT(x->shape[d] == y->shape[d], BF_STATUS_INVALID_SHAPE);
+	BFarray const* const ops[3] = {x, y, sk};
+	BFB_ASSERT(nd >= 1 && rows_match(ops, nd - 1, {1, 1, 1}), BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(y->shape[nd-1] == x->shape[nd-1], BF_STATUS_INVALID_SHAPE);
 	const long ntime = x->shape[nd-1];
 	const long M = plan->window;
 	const long nwin = div_up(ntime, M);
-	if( sk ) {
-		BFB_ASSERT(sk->ndim == nd, BF_STATUS_INVALID_SHAPE);
-		for( int d=0; d<nd-1; ++d ) BFB_ASSERT(sk->shape[d] == x->shape[d], BF_STATUS_INVALID_SHAPE);
-		BFB_ASSERT(sk->shape[nd-1] == nwin, BF_STATUS_INVALID_SHAPE);
-	}
-	const long isz = dtype_nbyte(x->dtype);
-	BFB_ASSERT(x->strides[nd-1] == isz && y->strides[nd-1] == isz, BF_STATUS_UNSUPPORTED_STRIDE);
-	BFB_ASSERT((uintptr_t)x->data % isz == 0 && (uintptr_t)y->data % isz == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	for( int d=0; d<nd-1; ++d )
-		BFB_ASSERT(x->strides[d] % isz == 0 && y->strides[d] % isz == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	if( sk ) {
-		BFB_ASSERT(sk->strides[nd-1] == 4 && (uintptr_t)sk->data % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-		for( int d=0; d<nd-1; ++d ) BFB_ASSERT(sk->strides[d] % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
-	}
-	long nrows = 1;
-	for( int d=0; d<nd-1; ++d ) {
-		BFB_ASSERT(x->shape[d] <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
-		nrows *= x->shape[d];
-		BFB_ASSERT(nrows <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
-	}
+	BFB_ASSERT(!sk || sk->shape[nd-1] == nwin, BF_STATUS_INVALID_SHAPE);
+	SkParams P = {};
+	long nrows;
+	BFstatus s = row_batch(ops, nd - 1, &P.rows, &nrows);
+	if( s != BF_STATUS_SUCCESS ) return s;
 	// rows, windows and sample indices are 32-bit in the kernels
+	for( long d=0, n=1; d<nd-1; ++d ) {
+		BFB_ASSERT(x->shape[d] <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
+		n *= x->shape[d];
+		BFB_ASSERT(n <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
+	}
 	BFB_ASSERT(ntime + M <= INT_MAX && nrows * nwin <= INT_MAX, BF_STATUS_UNSUPPORTED_SHAPE);
 
 	const size_t nrec = (size_t)nrows * nwin;
 	const size_t off_flag = round_up<size_t>(nrec * sizeof(double), SK_ALIGN);
-	const size_t need = std::max<size_t>(off_flag + round_up<size_t>(nrec, SK_ALIGN), SK_ALIGN);
-	if( exec_storage_size ) {
-		if( !exec_storage ) { *exec_storage_size = need; return BF_STATUS_SUCCESS; }
-		BFB_ASSERT(*exec_storage_size >= need, BF_STATUS_INSUFFICIENT_STORAGE);
-	} else {
-		BFB_ASSERT(!exec_storage, BF_STATUS_INVALID_ARGUMENT);
-		if( plan->own_size < need ) {
-			if( plan->own_ws ) cudaFree(plan->own_ws);
-			plan->own_ws = nullptr; plan->own_size = 0;
-			BFB_CUDA(cudaMalloc(&plan->own_ws, need), BF_STATUS_MEM_ALLOC_FAILED);
-			plan->own_size = need;
-		}
-		exec_storage = plan->own_ws;
-	}
+	void* mem;
+	s = use_storage(plan->ws, std::max<size_t>(off_flag + round_up<size_t>(nrec, SK_ALIGN), SK_ALIGN),
+	                exec_storage, exec_storage_size, &mem);
+	if( s != BF_STATUS_SUCCESS || !mem ) return s;
 	if( nrows == 0 || ntime == 0 ) return BF_STATUS_SUCCESS;
 
-	SkParams P = {};
 	P.in  = (const char*)x->data;
 	P.out = (char*)y->data;
-	P.sk  = sk ? (float*)sk->data : nullptr;
-	P.nrowdim = nd - 1;
-	for( int d=0; d<nd-1; ++d ) {
-		P.rshape[d]  = (int)x->shape[d];
-		P.xstride[d] = x->strides[d];
-		P.ystride[d] = y->strides[d];
-		P.kstride[d] = sk ? sk->strides[d] / 4 : 0;
-	}
+	P.sk  = sk ? (char*)sk->data : nullptr;
 	P.ntime = (int)ntime;
 	P.M     = (int)M;
 	P.nwin  = (int)nwin;
 	P.nrows = (int)nrows;
+	const long isz = dtype_nbyte(x->dtype);
 	// about four 16-byte loads per lane: the smallest power of two of lanes
 	// with at least a quarter of a window's chunks each, at most a warp
 	const long chunks = div_up(M * isz, 16L);
@@ -404,7 +360,7 @@ BFstatus sk_execute(BFskflag plan, BFarray const* x, BFarray const* y, BFarray c
 	bool same = x->data == y->data;
 	for( int d=0; d<nd-1; ++d ) same = same && x->strides[d] == y->strides[d];
 	P.inplace = same;
-	char* ws = (char*)exec_storage;
+	char* ws = (char*)mem;
 	P.s1   = (double*)ws;
 	P.flag = (unsigned char*)(ws + off_flag);
 
@@ -422,12 +378,7 @@ BFstatus sk_execute(BFskflag plan, BFarray const* x, BFarray const* y, BFarray c
 
 extern "C" {
 
-BFstatus bfSkFlagCreate(BFskflag* plan_ptr) {
-	BFB_ASSERT(plan_ptr, BF_STATUS_INVALID_POINTER);
-	*plan_ptr = nullptr;
-	BFB_TRY(*plan_ptr = new BFskflag_impl());
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfSkFlagCreate(BFskflag* plan_ptr) { return create_handle(plan_ptr); }
 
 BFstatus bfSkFlagInit(BFskflag plan, int window, int nacc, double shape, double lo, double hi) {
 	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
@@ -449,10 +400,6 @@ BFstatus bfSkFlagExecute(BFskflag plan, BFarray const* x, BFarray const* y, BFar
 	BFB_TRY(return sk_execute(plan, x, y, sk, exec_storage, exec_storage_size));
 }
 
-BFstatus bfSkFlagDestroy(BFskflag plan) {
-	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
-	delete plan;
-	return BF_STATUS_SUCCESS;
-}
+BFstatus bfSkFlagDestroy(BFskflag plan) { return destroy_handle(plan); }
 
 } // extern "C"

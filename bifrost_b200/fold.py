@@ -10,7 +10,7 @@ import ctypes
 
 import numpy as np
 
-from bifrost_b200.libbifrost import _bf, _check, _get, BifrostObject
+from bifrost_b200.libbifrost import _bf, _check, _exec_storage, BifrostObject
 from bifrost_b200.ndarray import asarray
 from bifrost_b200.coherent_dedisp import KDM
 
@@ -41,21 +41,21 @@ class Fold(BifrostObject):
         self.tsamp, self.t0 = float(tsamp), float(t0)
         self.nu, self.nudot, self.nuddot = float(nu), float(nudot), float(nuddot)
 
+    def _run(self, idata, odata, count, first, accumulate, **storage):
+        return _exec_storage(_bf.bfFoldExecute, self.obj, asarray(idata).as_BFarray(), int(first),
+                             asarray(odata).as_BFarray(), asarray(count).as_BFarray(), int(bool(accumulate)),
+                             **storage)
+
     def execute(self, idata, odata, count, first=0, accumulate=False):
         """Fold idata, whose sample 0 is stream sample `first`, into odata (f32
         sums) and count (i32): overwrite them, or add to them with
         accumulate=True."""
-        _check(_bf.bfFoldExecute(self.obj, asarray(idata).as_BFarray(), int(first), asarray(odata).as_BFarray(),
-                                 asarray(count).as_BFarray(), int(bool(accumulate)), None, None))
+        self._run(idata, odata, count, first, accumulate)
         return odata
 
     def get_workspace_size(self, idata, odata, count):
-        return _get(_bf.bfFoldExecute, self.obj, asarray(idata).as_BFarray(), 0, asarray(odata).as_BFarray(),
-                    asarray(count).as_BFarray(), 0, None)
+        return self._run(idata, odata, count, 0, False, query=True)
 
     def execute_workspace(self, idata, odata, count, workspace_ptr, workspace_size, first=0, accumulate=False):
-        size = _bf.BFsize(workspace_size)
-        _check(_bf.bfFoldExecute(self.obj, asarray(idata).as_BFarray(), int(first), asarray(odata).as_BFarray(),
-                                 asarray(count).as_BFarray(), int(bool(accumulate)), workspace_ptr,
-                                 ctypes.byref(size)))
+        self._run(idata, odata, count, first, accumulate, workspace=(workspace_ptr, workspace_size))
         return odata

@@ -6,7 +6,7 @@ S/N over the boxcar widths: out [..., ndm, nblk, 3] f32 holding
 (snr, start offset in the block, width)."""
 import ctypes
 
-from bifrost_b200.libbifrost import _bf, _check, _get, BifrostObject
+from bifrost_b200.libbifrost import _bf, _check, _exec_storage, BifrostObject
 from bifrost_b200.ndarray import asarray
 
 
@@ -26,18 +26,17 @@ class PulseSearch(BifrostObject):
         _check(_bf.bfPulseSearchInit(self.obj, len(widths), arr, int(decim)))
         self.widths, self.decim = widths, int(decim)
 
+    def _run(self, idata, odata, **storage):
+        return _exec_storage(_bf.bfPulseSearchExecute, self.obj, asarray(idata).as_BFarray(),
+                             asarray(odata).as_BFarray(), **storage)
+
     def execute(self, idata, odata):
-        _check(_bf.bfPulseSearchExecute(self.obj, asarray(idata).as_BFarray(),
-                                        asarray(odata).as_BFarray(), None, None))
+        self._run(idata, odata)
         return odata
 
     def get_workspace_size(self, idata, odata):
-        return _get(_bf.bfPulseSearchExecute, self.obj, asarray(idata).as_BFarray(),
-                    asarray(odata).as_BFarray(), None)
+        return self._run(idata, odata, query=True)
 
     def execute_workspace(self, idata, odata, workspace_ptr, workspace_size):
-        size = _bf.BFsize(workspace_size)
-        _check(_bf.bfPulseSearchExecute(self.obj, asarray(idata).as_BFarray(),
-                                        asarray(odata).as_BFarray(), workspace_ptr,
-                                        ctypes.byref(size)))
+        self._run(idata, odata, workspace=(workspace_ptr, workspace_size))
         return odata

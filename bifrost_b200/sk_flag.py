@@ -5,10 +5,9 @@ For each row of x [..., ntime] (u8, u16 or f32 power) and each window of
 `window` samples, the spectral kurtosis estimator sk; windows outside
 [lo, hi] are replaced by the mean of the row's clean samples.  y has x's
 dtype and shape and may be x itself."""
-import ctypes
 import math
 
-from bifrost_b200.libbifrost import _bf, _check, _get, BifrostObject
+from bifrost_b200.libbifrost import _bf, _check, _exec_storage, BifrostObject
 from bifrost_b200.ndarray import asarray
 
 
@@ -53,19 +52,19 @@ class SkFlag(BifrostObject):
         self.window, self.nacc, self.shape = int(window), int(nacc), float(shape)
         self.lo, self.hi = float(lo), float(hi)
 
+    def _run(self, idata, odata, sk, **storage):
+        return _exec_storage(_bf.bfSkFlagExecute, self.obj, asarray(idata).as_BFarray(),
+                             asarray(odata).as_BFarray(), _arr(sk), **storage)
+
     def execute(self, idata, odata, sk=None):
         """y = odata (may be idata) from x = idata; sk, if given, receives the
         f32 [..., nwin] statistic."""
-        _check(_bf.bfSkFlagExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
-                                   _arr(sk), None, None))
+        self._run(idata, odata, sk)
         return odata
 
     def get_workspace_size(self, idata, odata, sk=None):
-        return _get(_bf.bfSkFlagExecute, self.obj, asarray(idata).as_BFarray(),
-                    asarray(odata).as_BFarray(), _arr(sk), None)
+        return self._run(idata, odata, sk, query=True)
 
     def execute_workspace(self, idata, odata, workspace_ptr, workspace_size, sk=None):
-        size = _bf.BFsize(workspace_size)
-        _check(_bf.bfSkFlagExecute(self.obj, asarray(idata).as_BFarray(), asarray(odata).as_BFarray(),
-                                   _arr(sk), workspace_ptr, ctypes.byref(size)))
+        self._run(idata, odata, sk, workspace=(workspace_ptr, workspace_size))
         return odata

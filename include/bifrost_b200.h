@@ -205,7 +205,9 @@ BFstatus bfReduce(BFarray const* in, BFarray const* out, BFreduce_op op);
  * of row d are left untouched (ref: src/fdmt.cu:120-124,702-708).
  * Storage protocol for plan_storage / exec_storage (fdmt.h:71-78,108-115):
  *   (NULL, NULL)  library-managed;  (NULL, &size) query only;
- *   (ptr,  &size) caller-provided.
+ *   (ptr,  &size) caller-provided, at least the queried size
+ *   (BF_STATUS_INSUFFICIENT_STORAGE otherwise);  (ptr, NULL) is refused
+ *   (BF_STATUS_INVALID_ARGUMENT).
  * ------------------------------------------------------------------ */
 typedef struct BFfdmt_impl* BFfdmt;
 
@@ -341,8 +343,7 @@ BFstatus bfVisibilitiesFromStorage(BFarray const* in, BFarray const* out);
  * argmax of b_w, s_w = (b_w[t_w] - mu_w) / sigma_w (0 when sigma_w = 0), and
  * the block reports the first width with the largest s_w as
  * (s_w, t_w - j decim, w).  Deterministic: no atomics, fixed merge order.
- * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
- * (NULL, &size) query only, (ptr, &size) caller-provided. */
+ * exec_storage follows the FDMT's storage protocol (above). */
 typedef struct BFpulsesearch_impl* BFpulsesearch;
 
 BFstatus bfPulseSearchCreate(BFpulsesearch* plan);
@@ -371,8 +372,7 @@ BFstatus bfPulseSearchDestroy(BFpulsesearch plan);
  * flagged).  y = x on clean windows; on flagged ones the row's fill, the fp64
  * sum of S1 over clean windows (ascending) over their sample count (0 if none),
  * rounded to nearest even into the dtype.  Deterministic: no atomics.
- * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
- * (NULL, &size) query only, (ptr, &size) caller-provided.
+ * exec_storage follows the FDMT's storage protocol (above).
  * BF_STATUS_UNSUPPORTED_SHAPE when rows, rows x windows or ntime + M exceed
  * 2^31 - 1. */
 typedef struct BFskflag_impl* BFskflag;
@@ -411,8 +411,7 @@ BFstatus bfSkFlagDestroy(BFskflag plan);
  * out cf32, same shape, time unit stride; only written; must not overlap in.
  * N <= 4096 runs one fused kernel; longer N run bfFft through plans the
  * handle owns.  Deterministic: no atomics.  exec_storage follows the FDMT's
- * protocol: (NULL, NULL) library-managed, (NULL, &size) query only,
- * (ptr, &size) caller-provided. */
+ * storage protocol (above). */
 typedef struct BFcoherentdedisp_impl* BFcoherentdedisp;
 
 BFstatus bfCoherentDedispCreate(BFcoherentdedisp* plan);
@@ -452,8 +451,7 @@ BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan);
  * poisons only its own bin.  Counts must stay below 2^31.
  * BF_STATUS_UNSUPPORTED_SHAPE when rows or ntime exceed 32 bits.  ntime = 0
  * or no rows is a no-op that, with accumulate = 0, still zeroes out and count.
- * exec_storage follows the FDMT's protocol: (NULL, NULL) library-managed,
- * (NULL, &size) query only, (ptr, &size) caller-provided. */
+ * exec_storage follows the FDMT's storage protocol (above). */
 typedef struct BFfold_impl* BFfold;
 
 BFstatus bfFoldCreate(BFfold* plan);
