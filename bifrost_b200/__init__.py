@@ -6,6 +6,7 @@ that the per-gulp path uses: ``bf.ndarray``/``asarray``/``empty``/..., the op
 wrappers ``bf.transpose``, ``bf.reduce``, ``bf.fft.Fft``, ``bf.fdmt.Fdmt``,
 ``bf.pulse_search.PulseSearch``, ``bf.sk_flag.SkFlag``,
 ``bf.coherent_dedisp.CoherentDedisp``, ``bf.fold.Fold``,
+``bf.period_search.PeriodSearch``,
 ``bf.linalg.LinAlg``, ``bf.unpack``, ``bf.map`` (fixed-kernel subset) and the
 block classes in ``bf.blocks``.
 """
@@ -15,7 +16,8 @@ from bifrost_b200.DataType import DataType
 from bifrost_b200.Space import Space
 from bifrost_b200.ndarray import (ndarray, asarray, empty, zeros, empty_like,
                                   zeros_like, copy_array, memset_array)
-from bifrost_b200 import fdmt, fft, linalg, visibilities, pulse_search, sk_flag, coherent_dedisp, fold
+from bifrost_b200 import fdmt, fft, linalg, visibilities, pulse_search, sk_flag, coherent_dedisp, fold, \
+    period_search
 from bifrost_b200.reduce import reduce
 from bifrost_b200.transpose import transpose
 from bifrost_b200.unpack import unpack

@@ -352,6 +352,40 @@ BFstatus bfPulseSearchExecute(BFpulsesearch plan, BFarray const* in, BFarray con
                               void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfPulseSearchDestroy(BFpulsesearch plan);
 
+/* Periodicity search of a dispersion bank's spectra: whitened power with
+ * incoherent harmonic sums.
+ * in  [..., nbin] cf32 in device space (the r2c bfFft of each DM trial's
+ *     time series), bin unit stride, the base and every other stride
+ *     multiples of 8 bytes; each leading index is one row.
+ * out [..., nlevel, nblk, 2] f32, the leading dims of in, last axis unit
+ *     stride, other strides multiples of 4 bytes; only written.
+ * Init: nharm in {1, 2, 4, 8, 16, 32}, 16 <= window <= 8192,
+ * 1 <= decim <= 2^24 (BF_STATUS_INVALID_ARGUMENT otherwise); host work only.
+ * nlevel = log2(nharm) + 1, nblk = ceil(nbin / decim).  Per row, every fp64
+ * step one round-to-nearest operation:
+ *   P[k] = re re + im im (fp64, re and im widened from f32);
+ *   window j = bins [j window, min((j+1) window, nbin)), med_j the element of
+ *   rank floor((m_j - 1) / 2) of its m_j values of P (the lower median);
+ *   p[0] = 0; p[k] = (float)((P[k] / med_j) LN2) if med_j > 0, else 0, with
+ *   LN2 = 0.6931471805599453 (noise gives p close to Exp(1));
+ *   S_1[k] = p[k]; S_h[k] = S_{h/2}[k] + T_h[k] for h = 2, 4, .., nharm, T_h[k]
+ *   the fp64 sum over odd i < h ascending of p[(2 i k + h) / (2 h)] (integer
+ *   division: k is the highest harmonic, the fundamental is at k / h);
+ *   block j of level l (h = 2^l) covers bins [j decim, min((j+1) decim, nbin))
+ *   and reports its first k with the largest S_h as
+ *   out[..., l, j, :] = ((float)S_h[k], k - j decim).
+ * A NaN or inf in a row leaves that row's values unspecified and every other
+ * row alone.  BF_STATUS_UNSUPPORTED_SHAPE unless 1 <= nbin <= 2^24 + 1 and
+ * rows <= 2^31 - 1.  Deterministic: no atomics, fixed reduction order.
+ * exec_storage follows the FDMT's storage protocol (above). */
+typedef struct BFperiodsearch_impl* BFperiodsearch;
+
+BFstatus bfPeriodSearchCreate(BFperiodsearch* plan);
+BFstatus bfPeriodSearchInit(BFperiodsearch plan, int nharm, int window, int decim);
+BFstatus bfPeriodSearchExecute(BFperiodsearch plan, BFarray const* in, BFarray const* out,
+                               void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfPeriodSearchDestroy(BFperiodsearch plan);
+
 /* RFI excision by windowed spectral kurtosis (SK), for power filterbanks in
  * front of the FDMT.
  * x [..., ntime] u8, u16 or f32 power (i8 and every other dtype:

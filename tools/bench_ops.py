@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,period_search,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -278,6 +278,9 @@ def main():
 
     if 'fold' in ops:
         bench_fold(stream)
+
+    if 'period_search' in ops:
+        bench_period_search(stream)
 
 
 def gpu_name():
@@ -877,6 +880,114 @@ def bench_fold(stream, nrep=10):
         torch.cuda.empty_cache()
 
 
+def bench_period_search(stream, nrep=20):
+    """bfPeriodSearchExecute on the config-2 bank shape: 794 x 131072 f32 of
+    seeded noise with a periodic pulse train in a few rows, through a bfFft r2c
+    to [794, 65537] cf32, then nharm 32, window 1024, decim 64.  The bfFft, the
+    search and a torch composition of the same definition (torch.fft.rfft, a
+    lower median over unfolded windows, fp64 gather sums, block maxima) are
+    timed alternately in one loop; a torch.profiler run of its own splits the
+    search by kernel.  Shape bound: the cf32 spectrum read, p written and read
+    once, and the peak map written, at 3.35 TB/s (H100 SXM data sheet, 700 W).
+    Two runs are compared bit for bit.  The torch composition transforms
+    with cuFFT, whose spectrum differs from bfFft's in the last bits, so its
+    output is timed but not compared."""
+    from torch.profiler import ProfilerActivity, profile
+    print(json.dumps({'op': 'period_search.device', 'gpu': gpu_name()}), flush=True)
+    nrow, ntime, nharm, window, decim = 794, 131072, 32, 1024, 64
+    nbin = ntime // 2 + 1
+    nlevel = nharm.bit_length()
+    nblk = bf.period_search.output_nblock(nbin, decim)
+    gen = torch.Generator(device='cuda').manual_seed(1234)
+    xt = torch.randn(nrow, ntime, generator=gen, device='cuda', dtype=torch.float32)
+    period = 517.3                                              # samples: fundamental at 253.4 bins
+    pulses = torch.arange(0, ntime - 1, period, device='cuda').round().long()
+    for r in (100, 400, 700):
+        xt[r, pulses] += 3.0
+    x = bf.asarray(xt)
+    spec = bf.empty((nrow, nbin), 'cf32', 'cuda')
+    fft = bf.fft.Fft()
+    fft.init(x, spec, axes=1)
+    plan = bf.period_search.PeriodSearch()
+    plan.init(nharm, window, decim)
+    d_a = bf.zeros((nrow, nlevel, nblk, 2), 'f32', 'cuda')
+    d_b = bf.zeros((nrow, nlevel, nblk, 2), 'f32', 'cuda')
+
+    ln2 = 0.6931471805599453
+    kk = torch.arange(nbin, device='cuda', dtype=torch.int64)
+    gathers = [[(2 * i * kk + (1 << l)) // (2 << l) for i in range(1, 1 << l, 2)] for l in range(1, nlevel)]
+
+    def torch_search():
+        X = torch.fft.rfft(xt, dim=1)
+        P = X.real.double() ** 2 + X.imag.double() ** 2
+        full = (nbin // window) * window
+        med = torch.median(P[:, :full].unfold(1, window, window), dim=2).values
+        med = med.repeat_interleave(window, dim=1)
+        if full < nbin:
+            med = torch.cat([med, torch.median(P[:, full:], dim=1, keepdim=True).values.expand(-1, nbin - full)], 1)
+        p = torch.where(med > 0, ((P / med) * ln2).float(), torch.zeros((), device='cuda'))
+        p[:, 0] = 0
+        p64 = p.double()
+        S = [p64]
+        for idx in gathers:
+            t = torch.zeros_like(p64)
+            for g in idx:
+                t = t + p64[:, g]
+            S.append(S[-1] + t)
+        pad = nblk * decim - nbin
+        out = torch.empty(nrow, nlevel, nblk, 2, device='cuda')
+        for l, s in enumerate(S):
+            sp = torch.nn.functional.pad(s, (0, pad), value=-float('inf')).view(nrow, nblk, decim)
+            v, i = sp.max(dim=2)
+            out[:, l, :, 0] = v.float()
+            out[:, l, :, 1] = i.float()
+        return out
+
+    fns = {'fft': lambda: fft.execute(x, spec),
+           'search': lambda: plan.execute(spec, d_a),
+           'torch': torch_search}
+    for _ in range(3):
+        for fn in fns.values():
+            fn()
+    torch.cuda.synchronize()
+    times = {k: [] for k in fns}
+    for _ in range(nrep):
+        for key, fn in fns.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            fn()
+            e1.record(stream)
+            torch.cuda.synchronize()
+            times[key].append(e0.elapsed_time(e1))
+    plan.execute(spec, d_b)
+    torch.cuda.synchronize()
+    a, b = np.asarray(d_a.copy('system')), np.asarray(d_b.copy('system'))
+    ms = {k: float(np.median(v)) for k, v in times.items()}
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(nrep):
+            plan.execute(spec, d_a)
+        torch.cuda.synchronize()
+    per_kernel = {}
+    for e in prof.key_averages():
+        if 'period_search' in e.key:
+            per_kernel[e.key.split('(')[0].split('<')[0].split()[-1]] = round(
+                e.device_time_total / max(e.count, 1) / 1e3, 4)
+
+    nbytes = nrow * nbin * 8 + 2 * nrow * nbin * 4 + nrow * nlevel * nblk * 2 * 4
+    sig = np.stack([bf.period_search.significance(a[:, l, :, 0], 1 << l) for l in range(nlevel)], axis=1)
+    r, l, j = np.unravel_index(int(np.argmax(sig)), sig.shape)
+    report('period_search cf32 %dx%d nharm=%d window=%d decim=%d' % (nrow, nbin, nharm, window, decim),
+           ms['search'], nbytes, bound_ms=round(nbytes / 3.35e12 * 1e3, 4),
+           hbm_share=round(nbytes / 3.35e12 * 1e3 / ms['search'], 3), kernels_ms=per_kernel,
+           fft_ms=round(ms['fft'], 4), torch_ms=round(ms['torch'], 4),
+           torch_over_search=round(ms['torch'] / ms['search'], 2),
+           identical=bool(np.array_equal(a.view(np.uint32), b.view(np.uint32))),
+           best=dict(row=int(r), nharm=1 << int(l), k=int(j) * decim + int(a[r, l, j, 1]),
+                     fundamental=round((int(j) * decim + int(a[r, l, j, 1])) / (1 << int(l)), 2),
+                     expected=round(ntime / period, 2), sigma=round(float(sig[r, l, j]), 2)))
+    del xt, x, spec, d_a, d_b
+
+
 if __name__ == '__main__':
     main()
-
