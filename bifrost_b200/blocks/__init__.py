@@ -1,6 +1,6 @@
 """Hot-path blocks with the call signatures of ``bifrost.blocks``
 (python/bifrost/blocks/*.py): copy, transpose, fft, detect, reduce,
-accumulate, fdmt, pulse_search, sk_flag, coherent_dedisp, fold, period_search, correlate, convert_visibilities, unpack -- plus ``spectrometer`` (the fused chain) and a
+accumulate, fdmt, pulse_search, sk_flag, coherent_dedisp, fold, period_search, write_candidates, correlate, convert_visibilities, unpack -- plus ``spectrometer`` (the fused chain) and a
 ``NumpySourceBlock`` / ``CallbackSinkBlock`` pair for feeding them."""
 from bifrost_b200.blocks.copy import copy, CopyBlock
 from bifrost_b200.blocks.transpose import transpose, TransposeBlock
@@ -14,6 +14,7 @@ from bifrost_b200.blocks.sk_flag import sk_flag, SkFlagBlock
 from bifrost_b200.blocks.coherent_dedisp import coherent_dedisp, CoherentDedispBlock
 from bifrost_b200.blocks.fold import fold, FoldBlock
 from bifrost_b200.blocks.period_search import period_search, PeriodSearchBlock
+from bifrost_b200.blocks.candidates import write_candidates, CandidatesSinkBlock
 from bifrost_b200.blocks.correlate import correlate, CorrelateBlock
 from bifrost_b200.blocks.convert_visibilities import convert_visibilities, ConvertVisibilitiesBlock
 from bifrost_b200.blocks.beamform import beamform, BeamformBlock

@@ -11,14 +11,16 @@ PEAK_FIELDS = ['snr', 'offset', 'width']
 def pulse_search_header(ihdr, widths, decim):
     """Output header of pulse_search(widths, decim) on a [..., trial, 'time']
     f32 sequence with header ihdr: the time axis (still the frame axis) steps
-    by decim samples and a last 'peak' axis of length 3 holds PEAK_FIELDS."""
+    by decim samples and a last 'peak' axis of length 3 holds PEAK_FIELDS.
+    `peak_decim` is decim, so a consumer can turn a frame and an offset back
+    into a sample of the searched series."""
     ohdr, t = H.derive(ihdr)
     H.check_time_frames(t, ('f32',), 'pulse_search', 'input')
     H.scale_step(t, len(t['shape']) - 1, decim)
     for key, value in (('shape', 3), ('labels', 'peak'), ('scales', None), ('units', None)):
         if key in t:
             t[key].append(value)
-    ohdr.update(boxcar_widths=[int(w) for w in widths], peak_fields=list(PEAK_FIELDS))
+    ohdr.update(boxcar_widths=[int(w) for w in widths], peak_fields=list(PEAK_FIELDS), peak_decim=int(decim))
     return ohdr
 
 

@@ -386,6 +386,43 @@ BFstatus bfPeriodSearchExecute(BFperiodsearch plan, BFarray const* in, BFarray c
                                void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfPeriodSearchDestroy(BFperiodsearch plan);
 
+/* Candidates: friends-of-friends clustering of a peak map over trial and time.
+ * peaks [..., ntrial, nblk, nfield] f32 in device space, nfield 2 or 3: field
+ *   0 the score (S/N of bfPulseSearch, power of bfPeriodSearch), field 1 the
+ *   offset in the block, field 2 (if present) carried along (the boxcar
+ *   width); field axis unit stride, every other stride and the base whole
+ *   elements.  Each leading index b is independent.
+ * table [..., ncap, 9] f64, last axis unit stride, other strides multiples of
+ *   8 bytes; count [..., 1] i32.  Both share the leading dims of peaks.
+ * Init: threshold finite, 0 <= trial_radius R_t <= 32, 1 <= decim <= 2^24,
+ * pos_radius R_p >= 0 with ceil(R_p / decim) <= 32 (BF_STATUS_INVALID_ARGUMENT
+ * otherwise); host work only.  Per leading index:
+ *   cell (t, j) is a member iff field0 >= threshold (fp64 compare) and
+ *   0 <= field1 < decim (so NaN in either field is never a member);
+ *   pos = fl64(j decim + field1), one fp64 addition rounded to nearest;
+ *   scan index k = j ntrial + t (time-major);
+ *   two members are friends iff |t - t'| <= R_t and |fl64(pos - pos')| <= R_p;
+ *   clusters are the connected components of the friendship graph, ordered
+ *   by the smallest k among their members;
+ *   each cluster's representative is its member with the largest field0, the
+ *   smaller k on ties (-0 and +0 tie).
+ * Row c < min(count, ncap) of table is the c-th cluster: (field0, t, pos,
+ * field2 or 0 of the representative, members, trial_lo, trial_hi, pos_lo,
+ * pos_hi); rows >= min(count, ncap) are left untouched.  count[..., 0] is the
+ * number of clusters, which may exceed ncap.  Every value is copied from peaks
+ * or is an integer, and the integer atomics it uses (min, max, add) do not
+ * depend on their order, so the output is the same in every run.  A fixed
+ * number of launches, no host synchronisation.  BF_STATUS_UNSUPPORTED_SHAPE
+ * unless ntrial nblk < 2^31 and nblk decim < 2^31.  exec_storage follows the
+ * FDMT's storage protocol (above). */
+typedef struct BFcandidates_impl* BFcandidates;
+
+BFstatus bfCandidatesCreate(BFcandidates* plan);
+BFstatus bfCandidatesInit(BFcandidates plan, double threshold, int trial_radius, int pos_radius, int decim);
+BFstatus bfCandidatesExecute(BFcandidates plan, BFarray const* peaks, BFarray const* table,
+                             BFarray const* count, void* exec_storage, BFsize* exec_storage_size);
+BFstatus bfCandidatesDestroy(BFcandidates plan);
+
 /* RFI excision by windowed spectral kurtosis (SK), for power filterbanks in
  * front of the FDMT.
  * x [..., ntime] u8, u16 or f32 power (i8 and every other dtype:

@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,period_search,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,period_search,candidates,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -281,6 +281,9 @@ def main():
 
     if 'period_search' in ops:
         bench_period_search(stream)
+
+    if 'candidates' in ops:
+        bench_candidates(stream)
 
 
 def gpu_name():
@@ -987,6 +990,79 @@ def bench_period_search(stream, nrep=20):
                      fundamental=round((int(j) * decim + int(a[r, l, j, 1])) / (1 << int(l)), 2),
                      expected=round(ntime / period, 2), sigma=round(float(sig[r, l, j]), 2)))
     del xt, x, spec, d_a, d_b
+
+
+
+def bench_candidates(stream, nrep=20):
+    """bfCandidatesExecute (trial_radius 8, pos_radius 256: the widest boxcar)
+    on the peak maps of the config-2 bank: the 794 x 131072 f32 output of the
+    config-2 bfFdmtExecute (bench.make_input, made on the device) through
+    bfPulseSearchExecute (widths 1..256 in powers of two) at decim 256 and 16,
+    at thresholds 6 and 5, plus one dense case (every cell a member, one
+    cluster).  The bound is the map's bytes at 3.35 TB/s (H100 SXM data sheet,
+    700 W).  The alternative it replaces, a device-to-host copy of the map and
+    oracle/candidates.py on the host, is timed once per case on the wall
+    clock and must give the same table.  Two runs are compared bit for bit."""
+    import time
+    import bench
+    from torch.profiler import ProfilerActivity, profile
+    from oracle import candidates as oc
+    print(json.dumps({'op': 'candidates.device', 'gpu': gpu_name()}), flush=True)
+    w = bench.workload(0)
+    d_in = bf.asarray(bench.make_input(w, 1), space='cuda')
+    md, ntime = w['max_delay'], w['ntime']
+    bank = bf.zeros((md, ntime), 'f32', 'cuda')
+    fplan = bf.fdmt.Fdmt()
+    fplan.init(w['nchan'], md, w['f0'], w['df'])
+    fplan.execute(d_in, bank)
+    bview = bank[:, :bench.NTIME_OUT]
+    widths, ncap = [1 << k for k in range(9)], 4096
+    for decim in (256, 16):
+        nblk = bf.pulse_search.output_nblock(bench.NTIME_OUT, widths, decim)
+        d_map = bf.zeros((md, nblk, 3), 'f32', 'cuda')
+        ps = bf.pulse_search.PulseSearch()
+        ps.init(widths, decim)
+        ps.execute(bview, d_map)
+        nbytes = md * nblk * 3 * 4
+        cases = [(6., False), (5., False)] + ([(-1e30, True)] if decim == 256 else [])
+        for threshold, dense in cases:
+            plan = bf.candidates.Candidates()
+            plan.init(threshold, 8, 256, decim)
+            tabs = [bf.zeros((ncap, 9), 'f64', 'cuda') for _ in range(2)]
+            cnts = [bf.zeros((1,), 'i32', 'cuda') for _ in range(2)]
+            ms = timeit(lambda: plan.execute(d_map, tabs[0], cnts[0]), nrep=nrep, stream=stream)
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(nrep):
+                    plan.execute(d_map, tabs[0], cnts[0])
+                torch.cuda.synchronize()
+            per_kernel = {e.key.split('(')[0].split()[-1].replace('bfb::', ''):
+                          round(e.device_time_total / max(e.count, 1) / 1e3, 4)
+                          for e in prof.key_averages() if 'candidates_' in e.key}
+            plan.execute(d_map, tabs[1], cnts[1])
+            torch.cuda.synchronize()
+            a, b = (np.asarray(x.copy('system')) for x in tabs)
+            count = int(np.asarray(cnts[0].copy('system'))[0])
+            t0 = time.perf_counter()
+            host = np.asarray(d_map.copy('system'))
+            t1 = time.perf_counter()
+            want = oc.cluster(host, threshold, 8, 256, decim)
+            t2 = time.perf_counter()
+            n = min(count, ncap)
+            report('candidates %dx%d decim=%d threshold=%s' % (md, nblk, decim, 'all' if dense else threshold),
+                   ms, nbytes, map_MB=round(nbytes / 1e6, 2), bound_ms=round(nbytes / 3.35e12 * 1e3, 4),
+                   share_of_bound=round(nbytes / 3.35e12 * 1e3 / ms, 3), kernels_ms=per_kernel,
+                   members=int(np.count_nonzero((host[..., 0].astype(np.float64) >= threshold))),
+                   clusters=count, host_copy_ms=round((t1 - t0) * 1e3, 2),
+                   host_cluster_ms=round((t2 - t1) * 1e3, 1),
+                   host_total_over_op=round((t2 - t0) * 1e3 / ms, 1),
+                   matches_host=bool(len(want) == count and np.array_equal(a[:n].view(np.uint64),
+                                                                           want[:n].view(np.uint64))),
+                   identical=bool(np.array_equal(a.view(np.uint64), b.view(np.uint64))),
+                   brightest=[[int(r[1]), int(r[2]), int(r[3]), round(float(r[0]), 2)]
+                              for r in a[:n][np.argsort(a[:n, 0])[::-1][:3]]])
+            del tabs, cnts
+        del d_map
+    del d_in, bank
 
 
 if __name__ == '__main__':
