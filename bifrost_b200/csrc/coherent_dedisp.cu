@@ -25,8 +25,16 @@
 //       coherent_dedisp_keep_kernel (the kept L samples of each segment).
 //
 // Both paths take phi_k from cd_chirp.  No atomics: two runs give the same bits.
+//
+// bfCoherentDedispFilterbank (the coherent filterbank) runs the same filter
+// with each fine channel's own top edge in the chirp, inverts each of the
+// nfine blocks of N / nfine bins on its own, and detects and sums nint samples
+// straight into f32: coherent_filterbank_fused_kernel for N <= 4096; gather,
+// bfFft, chirp, an inverse bfFft over the blocks and
+// coherent_filterbank_detect_kernel for longer N.
 #include "shape.hpp"
 #include "fft4096.cuh"
+#include "detect.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -54,11 +62,12 @@ struct CdParams {
 };
 
 // H_k / N = exp(2 pi i phi_k) / N for channel c: phi in fp64, reduced modulo
-// one turn before the rounding to fp32.
-__device__ __forceinline__ float2 cd_chirp(CdParams const& P, long c, int k) {
+// one turn before the rounding to fp32.  below: how far (MHz) the reference
+// edge lies under the channel's top edge (0, or cd_fine_below).
+__device__ __forceinline__ float2 cd_chirp(CdParams const& P, long c, int k, double below) {
 	const double fc  = P.f0 + (double)c * P.df;
 	const double adf = fabs(P.df);
-	const double top = fc + 0.5 * adf;
+	const double top = fc + 0.5 * adf - below;
 	const double nu  = (double)(k < P.N / 2 ? k : k - P.N) / (double)P.N * P.df;
 	double phi = P.K * (nu * (1.0 / (fc * fc) - 1.0 / (top * top)) - nu * nu / (fc * fc * (fc + nu)));
 	if( P.df < 0. ) phi = -phi;
@@ -67,6 +76,16 @@ __device__ __forceinline__ float2 cd_chirp(CdParams const& P, long c, int k) {
 	sincospi(2.0 * phi, &s, &co);
 	const double inv = 1.0 / (double)P.N;
 	return make_float2((float)(co * inv), (float)(s * inv));
+}
+
+// How far (MHz) the top edge of the fine channel holding bin k lies under the
+// coarse top edge, when the N bins split into nfine fine channels of N / nfine
+// bins: fine channel j holds bins (N/2 + j N/nfine + q) mod N, and its top
+// edge is f_c - df/2 + (j + 1/2) df' + |df'|/2 with df' = df / nfine.
+__device__ __forceinline__ double cd_fine_below(int N, double df, int nfine, int k) {
+	if( nfine == 1 ) return 0.;
+	const int j = ((k + N / 2) & (N - 1)) / (N / nfine);
+	return (double)(df > 0. ? nfine - 1 - j : j) * (fabs(df) / (double)nfine);
 }
 
 template<int KIND>
@@ -81,7 +100,9 @@ __device__ __forceinline__ float2 cd_load(const char* row, long t) {
 // --------------------------------------------------------------- fused path
 // Forward FFT of N = 256 R3 points across T = 16 R3 threads (fft_fast_kernel's
 // stages): thread p enters with x[p + T m] in v[m] and leaves with X[cd_index(s)]
-// in v[s].  tb: the twiddle bases, laid out as in fft_fast_kernel.
+// in v[s].  tb: the stage-2 twiddle bases [4][256], W_256^((p&15) 2^i), which
+// every transform length shares; tb3: the stage-3 bases [Q LOG][256] of this
+// length (fft_fast_kernel keeps both in one table).
 template<int R3>
 __device__ __forceinline__ int cd_index(int p, int s) {
 	constexpr int T = 16 * R3, Q = 16 / R3;
@@ -94,7 +115,7 @@ __device__ __forceinline__ int cd_index(int p, int s) {
 
 template<int R3>
 __device__ __forceinline__ void cd_fft(float (&vr)[16], float (&vi)[16], float2* buf,
-                                       const float2* tb, int tid, int p) {
+                                       const float2* tb, const float2* tb3, int tid, int p) {
 	constexpr int T = 16 * R3, Q = 16 / R3;
 	constexpr int LOG = (R3 == 16) ? 4 : (R3 == 8) ? 3 : (R3 == 4) ? 2 : (R3 == 2) ? 1 : 0;
 	// stage 1 (Ns = 1)
@@ -124,7 +145,7 @@ __device__ __forceinline__ void cd_fft(float (&vr)[16], float (&vi)[16], float2*
 		float ar[R3], ai[R3];
 #pragma unroll
 		for( int m=0; m<R3; ++m ) { ar[m] = vr[q + Q * m]; ai[m] = vi[q + Q * m]; }
-		fast_twiddle<R3>(ar, ai, tb + (4 + q * LOG) * 256 + tid);
+		fast_twiddle<R3>(ar, ai, tb3 + q * LOG * 256 + tid);
 		SDft<R3>::apply(ar, ai);
 #pragma unroll
 		for( int t=0; t<R3; ++t ) { or_[q * R3 + t] = ar[t]; oi_[q * R3 + t] = ai[t]; }
@@ -158,7 +179,7 @@ coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
 	for( int q=0; q<Q; ++q )
 #pragma unroll
 		for( int i=0; i<LOG; ++i ) tb[(4 + q * LOG + i) * 256 + tid] = cd_twiddle((((p + T * q) & 255) << i) & (N - 1), N);
-	for( int k=tid; k<N; k+=256 ) chirp[k] = cd_chirp(P, c, k);
+	for( int k=tid; k<N; k+=256 ) chirp[k] = cd_chirp(P, c, k, 0.);
 	// (the first barrier inside cd_fft publishes both tables)
 	const long nline = P.nbatch * P.nseg;
 	for( long L0 = (long)blockIdx.x * G; L0 < nline; L0 += (long)gridDim.x * G ) {
@@ -177,7 +198,7 @@ coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
 			if( live && t < P.ntime ) v = cd_load<KIND>(irow, t);
 			vr[m] = v.x; vi[m] = v.y;
 		}
-		cd_fft<R3>(vr, vi, buf, tb, tid, p);
+		cd_fft<R3>(vr, vi, buf, tb, tb + 4 * 256, tid, p);
 		// z = conj(H X / N) into natural order for the second transform
 		__syncthreads();                          // every read of the last stage is done
 #pragma unroll
@@ -189,7 +210,7 @@ coherent_dedisp_fused_kernel(const __grid_constant__ CdParams P) {
 		__syncthreads();
 #pragma unroll
 		for( int m=0; m<16; ++m ) { const float2 v = buf[spad(p + T * m)]; vr[m] = v.x; vi[m] = v.y; }
-		cd_fft<R3>(vr, vi, buf, tb, tid, p);
+		cd_fft<R3>(vr, vi, buf, tb, tb + 4 * 256, tid, p);
 		if( live ) {
 			float2* orow = (float2*)(P.out + off[1]);
 			const long keep = min((long)P.L, P.ntime - t0);
@@ -223,12 +244,12 @@ coherent_dedisp_gather_kernel(const __grid_constant__ CdParams P, long nrows) {
 }
 
 __global__ void __launch_bounds__(256)
-coherent_dedisp_chirp_kernel(const __grid_constant__ CdParams P, long nrows) {
+coherent_dedisp_chirp_kernel(const __grid_constant__ CdParams P, long nrows, int nfine) {
 	const long total = nrows * P.nseg * P.N;
 	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
 		const int k = (int)(i % P.N);
 		const long r = i / P.N / P.nseg;
-		const float2 h = cd_chirp(P, r / P.nbatch, k);
+		const float2 h = cd_chirp(P, r / P.nbatch, k, cd_fine_below(P.N, P.df, nfine, k));
 		const float2 x = P.ws[i];
 		P.ws[i] = make_float2(x.x * h.x - x.y * h.y, x.x * h.y + x.y * h.x);
 	}
@@ -246,6 +267,222 @@ coherent_dedisp_keep_kernel(const __grid_constant__ CdParams P, long nrows) {
 	}
 }
 
+// ------------------------------------------------------- coherent filterbank
+// bfCoherentDedispFilterbank: the dedispersed spectrum of each segment splits
+// into nfine blocks of Nf = N / nfine bins, each block runs its own inverse
+// Nf-point transform (fine channel j is block (j + nfine/2) mod nfine), and
+// the fine samples are detected and summed over nint straight into f32.
+struct CfbParams {
+	CdParams cd;                  // cd.L is the segment step S, cd.nbatch the nb rows
+	char* out;                    // f32 [nchan nfine, nprod or nb, ntime / (nfine nint)]
+	long os[3];                   // out strides, bytes
+	int  kind, mode, nfine, nint;
+};
+
+__device__ __forceinline__ float2 cd_load_any(int kind, const char* row, long t) {
+	switch( kind ) {
+	case CD_CF32: return cd_load<CD_CF32>(row, t);
+	case CD_CI8:  return cd_load<CD_CI8>(row, t);
+	case CD_CI16: return cd_load<CD_CI16>(row, t);
+	default:      return cd_load<CD_CI4>(row, t);
+	}
+}
+
+// The detected products of one fine sample: y alone (NPOL 1, scalar), or the
+// pair (x, y) in a polarised mode; as bfDetect computes them.
+template<int NPOL>
+__device__ __forceinline__ void cfb_detect(int mode, float2 x, float2 y, float (&o)[4]) {
+	if( NPOL == 1 ) { o[0] = mag2f(y); o[1] = o[2] = o[3] = 0.f; return; }
+	switch( mode ) {
+	case DET_STOKES:   detect_pol<DET_STOKES>(x, y, o); break;
+	case DET_STOKES_I: detect_pol<DET_STOKES_I>(x, y, o); o[1] = o[2] = o[3] = 0.f; break;
+	default:           detect_pol<DET_COHERENCE>(x, y, o); break;
+	}
+}
+
+// The nout outputs of one fine channel, one line and products pp, pp + 1 (pair):
+// output o sums fine samples o nint .. o nint + nint - 1 of the block staged at
+// blk (.x product pp, .y product pp + 1) left to right, as bfReduce does, and
+// goes to orow + o os[2] (product pp + 1 one os[1] further).
+__device__ __forceinline__ void cfb_store(CfbParams const& P, const float2* blk, char* orow, bool pair,
+                                          int nout, int nthread) {
+	for( int o = threadIdx.x; o < nout; o += nthread ) {
+		const int e = o * P.nint;
+		float2 a = blk[spad(e)];
+		for( int i=1; i<P.nint; ++i ) { const float2 v = blk[spad(e + i)]; a.x += v.x; a.y += v.y; }
+		char* out = orow + (long)o * P.os[2];
+		*(float*)out = a.x;
+		if( pair ) *(float*)(out + P.os[1]) = a.y;
+	}
+}
+
+// N = 256 R3 <= 4096 in one launch.  The forward transform, chirp and line
+// layout are coherent_dedisp_fused_kernel's; the inverse runs as G nfine
+// transforms of Nf = 256 R2 points (T2 = 16 R2 threads each), so thread (g, p)
+// stays on line g and holds fine block p / T2.  A CTA is NPOL halves of 256
+// threads, each with its own G transform buffers: in a polarised mode half 0
+// transforms x and half 1 y of the same lines, so the pair never has to sit in
+// one thread's registers (the reason for 512 threads and one CTA per SM there;
+// the scalar form keeps two CTAs of 256).  The detected products are staged in
+// the buffers, two per point, and summed over nint from there.
+template<int R3, int R2, int NPOL>
+__global__ void __launch_bounds__(256 * NPOL, 3 - NPOL)
+coherent_filterbank_fused_kernel(const __grid_constant__ CfbParams F) {
+	constexpr int N = 256 * R3, T = 16 * R3, G = 256 / T, Q = 16 / R3;
+	constexpr int LOG = (R3 == 16) ? 4 : (R3 == 8) ? 3 : (R3 == 4) ? 2 : (R3 == 2) ? 1 : 0;
+	constexpr int NF = 256 * R2, T2 = 16 * R2, Q2 = 16 / R2, NFINE = R3 / R2;
+	constexpr int LOG2 = (R2 == 16) ? 4 : (R2 == 8) ? 3 : (R2 == 4) ? 2 : (R2 == 2) ? 1 : 0;
+	constexpr int PITCH = N + (N >> 4) + 1, HALF = G * PITCH;
+	CdParams const& P = F.cd;
+	extern __shared__ __align__(16) unsigned char cd_smem[];
+	float2* const bufs = (float2*)cd_smem;           // [NPOL][G][PITCH] transform buffers
+	float2* tb    = bufs + NPOL * HALF;              // [4 + Q*LOG][256] twiddle bases
+	float2* tb2   = tb + 12 * 256;                   // [Q2*LOG2][256] stage-3 bases of the inverse
+	float2* chirp = tb2 + (R2 == R3 ? 0 : 8 * 256);  // [N] H_k / N, fine top edges
+	if( R2 == R3 ) tb2 = tb + 4 * 256;
+	const int h = threadIdx.x / 256, tid = threadIdx.x % 256, g = tid / T, p = tid % T;
+	const int p2 = tid % T2, blk = (tid / T2) % NFINE;
+	float2* const buf = bufs + h * HALF + g * PITCH;
+	float2* const sub = buf + spad(blk * NF);        // fine block blk of the line's buffer
+	const long c = blockIdx.y;
+	if( h == 0 ) {
+#pragma unroll
+		for( int i=0; i<4; ++i ) tb[i * 256 + tid] = cd_twiddle((R3 * ((p & 15) << i)) & (N - 1), N);
+#pragma unroll
+		for( int q=0; q<Q; ++q )
+#pragma unroll
+			for( int i=0; i<LOG; ++i )
+				tb[(4 + q * LOG + i) * 256 + tid] = cd_twiddle((((p + T * q) & 255) << i) & (N - 1), N);
+		if( R2 != R3 ) {
+#pragma unroll
+			for( int q=0; q<Q2; ++q )
+#pragma unroll
+				for( int i=0; i<LOG2; ++i )
+					tb2[(q * LOG2 + i) * 256 + tid] = cd_twiddle((((p2 + T2 * q) & 255) << i) & (NF - 1), NF);
+		}
+	}
+	for( int k=threadIdx.x; k<N; k+=256*NPOL ) chirp[k] = cd_chirp(P, c, k, cd_fine_below(N, P.df, NFINE, k));
+	// (the first barrier inside cd_fft publishes the tables)
+	const long S = P.L, q = (long)NFINE * F.nint;
+	const int nper = (int)(S / q);                   // outputs per fine channel and segment
+	const int nprod = NPOL == 1 ? 1 : detect_nprod(F.mode);
+	const int npair = (nprod + 1) / 2;               // staged product pairs, one per half
+	const long ngrp = P.nbatch / NPOL;               // scalar: the nb rows; polarised: one pair
+	const long nline = ngrp * P.nseg;
+	for( long L0 = (long)blockIdx.x * G; L0 < nline; L0 += (long)gridDim.x * G ) {
+		const long line = L0 + g;
+		const bool live = line < nline;
+		const long b = live ? line / P.nseg : 0;
+		const long t0 = live ? (line - b * P.nseg) * S : 0;
+		long off[2];
+		P.rows.offsets(c * P.nbatch + b * NPOL + h, off);
+		const char* irow = P.in + off[0];
+		float vr[16], vi[16];
+#pragma unroll
+		for( int m=0; m<16; ++m ) {
+			const long t = t0 + p + T * m;
+			float2 v = make_float2(0.f, 0.f);
+			if( live && t < P.ntime ) v = cd_load_any(F.kind, irow, t);
+			vr[m] = v.x; vi[m] = v.y;
+		}
+		cd_fft<R3>(vr, vi, buf, tb, tb + 4 * 256, tid, p);
+		__syncthreads();                          // every read of the last stage is done
+#pragma unroll
+		for( int s=0; s<16; ++s ) {
+			const int k = cd_index<R3>(p, s);
+			const float2 hk = chirp[k];
+			buf[spad(k)] = make_float2(vr[s] * hk.x - vi[s] * hk.y, -(vr[s] * hk.y + vi[s] * hk.x));
+		}
+		__syncthreads();
+		// the inverse of each fine block: conj(FFT_Nf(conj Y)) over its Nf bins
+#pragma unroll
+		for( int m=0; m<16; ++m ) { const float2 v = sub[spad(p2 + T2 * m)]; vr[m] = v.x; vi[m] = v.y; }
+		cd_fft<R2>(vr, vi, sub, tb, tb2, tid, p2);
+		__syncthreads();                          // every read of the buffers is done
+		if( NPOL == 1 ) {
+#pragma unroll
+			for( int s=0; s<16; ++s ) sub[spad(cd_index<R2>(p2, s))] = make_float2(mag2f(make_float2(vr[s], -vi[s])), 0.f);
+		} else {
+			// half 1 leaves y where half 0 finds it, at the same point of the other half's buffer
+			if( h == 1 ) {
+#pragma unroll
+				for( int s=0; s<16; ++s ) sub[spad(cd_index<R2>(p2, s))] = make_float2(vr[s], -vi[s]);
+			}
+			__syncthreads();
+			if( h == 0 ) {
+				float2* const suby = sub + HALF;
+#pragma unroll
+				for( int s=0; s<16; ++s ) {
+					const int e = spad(cd_index<R2>(p2, s));
+					float o[4];
+					cfb_detect<2>(F.mode, make_float2(vr[s], -vi[s]), suby[e], o);
+					sub[e] = make_float2(o[0], o[1]);
+					suby[e] = make_float2(o[2], o[3]);
+				}
+			}
+		}
+		__syncthreads();
+		// one line, product pair and fine channel at a time: consecutive threads
+		// write consecutive outputs, with no index arithmetic per output
+#pragma unroll 1
+		for( int gw=0; gw<G; ++gw ) {
+			const long lw = L0 + gw;
+			if( lw >= nline ) break;
+			const long bw = lw / P.nseg, sw = lw - bw * P.nseg;
+			const int nout = (int)(min(S, P.ntime - sw * S) / q);
+#pragma unroll 1
+			for( int pp=0; pp<npair; ++pp ) {
+				const float2* src = bufs + pp * HALF + gw * PITCH;
+				const bool pair = NPOL == 2 && 2 * pp + 1 < nprod;
+#pragma unroll 1
+				for( int jw=0; jw<NFINE; ++jw ) {
+					char* orow = F.out + (c * NFINE + jw) * F.os[0] + (NPOL == 1 ? bw : 2L * pp) * F.os[1] +
+					             sw * nper * F.os[2];
+					cfb_store(F, src + spad(((jw + NFINE / 2) % NFINE) * NF), orow, pair, nout, 256 * NPOL);
+				}
+			}
+		}
+	}
+}
+
+// Long path, after the inverse bfFft of every Nf-bin block in place: one thread
+// per (channel, row or pair, fine channel, output sample) reads fine channel j
+// from block (j + nfine/2) mod nfine of each segment and writes its products.
+template<int NPOL>
+__global__ void __launch_bounds__(256)
+coherent_filterbank_detect_kernel(const __grid_constant__ CfbParams F, long nrows) {
+	CdParams const& P = F.cd;
+	const long S = P.L, q = (long)F.nfine * F.nint, nper = S / q;
+	const long ngrp = P.nbatch / NPOL, nout = P.ntime / q;
+	const int Nf = P.N / F.nfine;
+	const int nprod = NPOL == 1 ? 1 : detect_nprod(F.mode);
+	const long total = nrows / NPOL * F.nfine * nout;
+	for( long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x ) {
+		const long tout = i % nout;
+		const long rj = i / nout;
+		const int j = (int)(rj % F.nfine);
+		const long rg = rj / F.nfine;                // channel c, group b
+		const long c = rg / ngrp, b = rg - c * ngrp;
+		const long s = tout / nper, o = tout - s * nper;
+		const int bk = (j + F.nfine / 2) % F.nfine;
+		const long r0 = c * P.nbatch + b * NPOL;     // the first ws row of the group
+		const float2* y = P.ws + ((r0 + NPOL - 1) * P.nseg + s) * P.N + (long)bk * Nf + o * F.nint;
+		const float2* x = P.ws + (r0 * P.nseg + s) * P.N + (long)bk * Nf + o * F.nint;
+		float a[4];
+		cfb_detect<NPOL>(F.mode, x[0], y[0], a);
+		for( int k=1; k<F.nint; ++k ) {
+			float d[4];
+			cfb_detect<NPOL>(F.mode, x[k], y[k], d);
+#pragma unroll
+			for( int u=0; u<4; ++u ) a[u] += d[u];
+		}
+		char* out = F.out + (c * F.nfine + j) * F.os[0] + tout * F.os[2];
+#pragma unroll
+		for( int u=0; u<4; ++u )
+			if( u < nprod ) *(float*)(out + (NPOL == 1 ? b : (long)u) * F.os[1]) = a[u];
+	}
+}
+
 } // namespace bfb
 
 using namespace bfb;
@@ -257,8 +494,11 @@ struct BFcoherentdedisp_impl {
 	BFfft  fft = nullptr;         // long path: one plan over [rows * nseg, N], run both ways
 	long   fft_lines = -1;
 	size_t fft_tmp = 0;
+	BFfft  fine = nullptr;        // filterbank long path: the inverse over [rows * nseg * nfine, N / nfine]
+	long   fine_lines = -1, fine_n = 0;
+	size_t fine_tmp = 0;
 	DeviceBuffer ws;
-	~BFcoherentdedisp_impl() { if( fft ) bfFftDestroy(fft); }
+	~BFcoherentdedisp_impl() { if( fft ) bfFftDestroy(fft); if( fine ) bfFftDestroy(fine); }
 };
 
 namespace {
@@ -287,21 +527,27 @@ BFarray cd_seg_array(void* data, long lines, long N) {
 	return a;
 }
 
-// (Re)plans the long path's transform for `lines` segments; sets fft_tmp.
-BFstatus cd_plan_fft(BFcoherentdedisp plan, long lines) {
-	if( plan->fft && plan->fft_lines == lines ) return BF_STATUS_SUCCESS;
-	if( !plan->fft ) {
-		BFstatus s = bfFftCreate(&plan->fft);
+// (Re)plans *fft over [lines, n] cf32 unless *planned == lines already; sets
+// *planned and *tmp.
+BFstatus cd_plan_lines(BFfft* fft, long* planned, size_t* tmp_size, long lines, long n) {
+	if( *fft && *planned == lines ) return BF_STATUS_SUCCESS;
+	if( !*fft ) {
+		BFstatus s = bfFftCreate(fft);
 		if( s != BF_STATUS_SUCCESS ) return s;
 	}
-	BFarray a = cd_seg_array(nullptr, lines, plan->nfft);
+	BFarray a = cd_seg_array(nullptr, lines, n);
 	int axis = 1;
 	size_t tmp = 0;
-	BFstatus s = bfFftInit(plan->fft, &a, &a, 1, &axis, 0, &tmp);
-	if( s != BF_STATUS_SUCCESS ) { plan->fft_lines = -1; return s; }
-	plan->fft_lines = lines;
-	plan->fft_tmp = tmp;
+	BFstatus s = bfFftInit(*fft, &a, &a, 1, &axis, 0, &tmp);
+	if( s != BF_STATUS_SUCCESS ) { *planned = -1; return s; }
+	*planned = lines;
+	*tmp_size = tmp;
 	return BF_STATUS_SUCCESS;
+}
+
+// (Re)plans the long path's transform for `lines` segments; sets fft_tmp.
+BFstatus cd_plan_fft(BFcoherentdedisp plan, long lines) {
+	return cd_plan_lines(&plan->fft, &plan->fft_lines, &plan->fft_tmp, lines, plan->nfft);
 }
 
 template<int KIND>
@@ -405,12 +651,171 @@ BFstatus cd_execute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out
 	const BFarray seg = cd_seg_array(P.ws, nrows * nseg, N);
 	s = bfFftExecute(plan->fft, &seg, &seg, 0, tmp, plan->fft_tmp);
 	if( s != BF_STATUS_SUCCESS ) return s;
-	coherent_dedisp_chirp_kernel<<<cd_grid(nws), 256, 0, st>>>(P, nrows);
+	coherent_dedisp_chirp_kernel<<<cd_grid(nws), 256, 0, st>>>(P, nrows, 1);
 	count_launch();
 	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 	s = bfFftExecute(plan->fft, &seg, &seg, 1, tmp, plan->fft_tmp);
 	if( s != BF_STATUS_SUCCESS ) return s;
 	coherent_dedisp_keep_kernel<<<cd_grid(nrows * ntime), 256, 0, st>>>(P, nrows);
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	return BF_STATUS_SUCCESS;
+}
+
+// ------------------------------------------------------- coherent filterbank
+template<int R3, int R2>
+void cfb_launch(CfbParams const& F, int npol, dim3 grid, size_t smem, cudaStream_t st) {
+	if( npol == 1 ) {
+		BFB_CUDA_THROW(cudaFuncSetAttribute(coherent_filterbank_fused_kernel<R3, R2, 1>,
+			cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), BF_STATUS_INTERNAL_ERROR);
+		coherent_filterbank_fused_kernel<R3, R2, 1><<<grid, 256, smem, st>>>(F);
+	} else {
+		BFB_CUDA_THROW(cudaFuncSetAttribute(coherent_filterbank_fused_kernel<R3, R2, 2>,
+			cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), BF_STATUS_INTERNAL_ERROR);
+		coherent_filterbank_fused_kernel<R3, R2, 2><<<grid, 512, smem, st>>>(F);
+	}
+}
+
+// R2 = R3 / nfine; the dead branches of short transforms instantiate nothing new
+template<int R3>
+void cfb_launch_r2(CfbParams const& F, int npol, dim3 grid, size_t smem, cudaStream_t st) {
+	switch( R3 / F.nfine ) {
+	case 1:  cfb_launch<R3, 1>(F, npol, grid, smem, st); break;
+	case 2:  cfb_launch<R3, (R3 < 2 ? R3 : 2)>(F, npol, grid, smem, st); break;
+	case 4:  cfb_launch<R3, (R3 < 4 ? R3 : 4)>(F, npol, grid, smem, st); break;
+	case 8:  cfb_launch<R3, (R3 < 8 ? R3 : 8)>(F, npol, grid, smem, st); break;
+	default: cfb_launch<R3, R3>(F, npol, grid, smem, st); break;
+	}
+}
+
+void cfb_launch_fused(CfbParams const& F, long nchan, int npol, cudaStream_t st) {
+	const int N = F.cd.N, R3 = N / 256;
+	const int G = 256 / (16 * R3);
+	const size_t smem = ((size_t)npol * G * (N + N / 16 + 1) + 12 * 256 + (F.nfine > 1 ? 8 * 256 : 0) + N) *
+	                    sizeof(float2);
+	int nsm = 132;
+	int dev = 0;
+	if( cudaGetDevice(&dev) == cudaSuccess ) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+	const long groups = div_up(F.cd.nbatch / npol * F.cd.nseg, (long)G);
+	const long per = std::max(1L, std::min(groups, div_up(8L * nsm, nchan)));
+	const dim3 grid((unsigned)per, (unsigned)nchan);
+	switch( R3 ) {
+	case 1:  cfb_launch_r2<1>(F, npol, grid, smem, st);  break;
+	case 2:  cfb_launch_r2<2>(F, npol, grid, smem, st);  break;
+	case 4:  cfb_launch_r2<4>(F, npol, grid, smem, st);  break;
+	case 8:  cfb_launch_r2<8>(F, npol, grid, smem, st);  break;
+	default: cfb_launch_r2<16>(F, npol, grid, smem, st); break;
+	}
+	count_launch();
+}
+
+BFstatus cfb_execute(BFcoherentdedisp plan, BFarray const* in, int nfine, int mode, int nint,
+                     BFarray const* out, void* exec_storage, BFsize* exec_storage_size) {
+	BFB_ASSERT(plan, BF_STATUS_INVALID_HANDLE);
+	BFB_ASSERT(in && out, BF_STATUS_INVALID_POINTER);
+	BFB_ASSERT(plan->planned, BF_STATUS_INVALID_STATE);
+	BFB_ASSERT(space_on_device(in->space) && space_on_device(out->space), BF_STATUS_UNSUPPORTED_SPACE);
+	const int kind = cd_kind(in->dtype);
+	BFB_ASSERT(kind >= 0 && out->dtype == BF_DTYPE_F32, BF_STATUS_UNSUPPORTED_DTYPE);
+	BFB_ASSERT(mode == DET_SCALAR || mode == DET_STOKES || mode == DET_STOKES_I || mode == DET_COHERENCE,
+	           BF_STATUS_UNSUPPORTED);
+	const long N = plan->nfft, L = N - plan->overlap;
+	BFB_ASSERT(nfine >= 1 && (nfine & (nfine - 1)) == 0 && N / nfine >= CD_NMIN, BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(nint >= 1 && (long)nfine * nint <= L, BF_STATUS_INVALID_ARGUMENT);
+	BFB_ASSERT(in->ndim == 3 && in->shape[0] == plan->nchan, BF_STATUS_INVALID_SHAPE);
+	const int npol = mode == DET_SCALAR ? 1 : 2;
+	const long nchan = plan->nchan, nb = in->shape[1], ntime = in->shape[2];
+	const long q = (long)nfine * nint;
+	BFB_ASSERT(npol == 1 || nb == 2, BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(ntime % q == 0, BF_STATUS_INVALID_SHAPE);
+	const long nprod = npol == 1 ? nb : detect_nprod(mode);
+	BFB_ASSERT(out->ndim == 3 && out->shape[0] == nchan * nfine && out->shape[1] == nprod &&
+	           out->shape[2] == ntime / q, BF_STATUS_INVALID_SHAPE);
+	BFB_ASSERT(nchan <= 65535, BF_STATUS_UNSUPPORTED_SHAPE);      // channels run on gridDim.y
+	CfbParams F = {};
+	CdParams& P = F.cd;
+	BFarray const* const ops[2] = {in, nullptr};
+	long nrows;
+	BFstatus s = row_batch(ops, 2, &P.rows, &nrows);
+	if( s != BF_STATUS_SUCCESS ) return s;
+	const bool empty = array_numel(out) == 0;
+	BFB_ASSERT(empty || (uintptr_t)out->data % 4 == 0, BF_STATUS_UNSUPPORTED_STRIDE);
+	for( int d=0; d<3; ++d ) {
+		BFB_ASSERT(empty || out->shape[d] <= 1 || (out->strides[d] > 0 && out->strides[d] % 4 == 0),
+		           BF_STATUS_UNSUPPORTED_STRIDE);
+		F.os[d] = out->strides[d];
+	}
+	const long S = q * (L / q);                   // the segment step: whole outputs per segment
+	const long nseg = div_up(ntime, S);
+	const bool fused = N <= CD_NFUSE;
+	const long nf = N / nfine;
+
+	size_t need = 0, seg_bytes = 0;
+	if( !fused && nrows * nseg > 0 ) {
+		seg_bytes = round_up<size_t>((size_t)(nrows * nseg * N) * 8, CD_ALIGN);
+		s = cd_plan_fft(plan, nrows * nseg);
+		if( s != BF_STATUS_SUCCESS ) return s;
+		size_t tmp = plan->fft_tmp;
+		if( nfine > 1 ) {
+			if( plan->fine_n != nf ) { plan->fine_lines = -1; plan->fine_n = nf; }
+			s = cd_plan_lines(&plan->fine, &plan->fine_lines, &plan->fine_tmp, nrows * nseg * nfine, nf);
+			if( s != BF_STATUS_SUCCESS ) return s;
+			tmp = std::max(tmp, plan->fine_tmp);
+		}
+		need = seg_bytes + round_up<size_t>(tmp, CD_ALIGN);
+	}
+	void* mem;
+	s = use_storage(plan->ws, std::max(need, CD_ALIGN), exec_storage, exec_storage_size, &mem);
+	if( s != BF_STATUS_SUCCESS || !mem ) return s;
+	if( nrows == 0 || ntime == 0 ) return BF_STATUS_SUCCESS;
+
+	P.in  = (const char*)in->data;
+	P.ntime  = ntime;
+	P.N      = (int)N;
+	P.L      = (int)S;
+	P.nseg   = nseg;
+	P.nbatch = nb;
+	P.f0 = plan->f0;
+	P.df = plan->df;
+	P.K  = CD_KDM * plan->dm * 1e6;
+	F.out   = (char*)out->data;
+	F.kind  = kind;
+	F.mode  = mode;
+	F.nfine = nfine;
+	F.nint  = nint;
+	cudaStream_t st = thread_stream();
+	if( fused ) {
+		cfb_launch_fused(F, nchan, npol, st);
+		BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+		return BF_STATUS_SUCCESS;
+	}
+	P.ws = (float2*)mem;
+	void* tmp = (char*)mem + seg_bytes;
+	const long nws = nrows * nseg * N;
+	switch( kind ) {
+	case CD_CF32: coherent_dedisp_gather_kernel<CD_CF32><<<cd_grid(nws), 256, 0, st>>>(P, nrows); break;
+	case CD_CI8:  coherent_dedisp_gather_kernel<CD_CI8><<<cd_grid(nws), 256, 0, st>>>(P, nrows);  break;
+	case CD_CI16: coherent_dedisp_gather_kernel<CD_CI16><<<cd_grid(nws), 256, 0, st>>>(P, nrows); break;
+	default:      coherent_dedisp_gather_kernel<CD_CI4><<<cd_grid(nws), 256, 0, st>>>(P, nrows);  break;
+	}
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	const BFarray seg = cd_seg_array(P.ws, nrows * nseg, N);
+	s = bfFftExecute(plan->fft, &seg, &seg, 0, tmp, plan->fft_tmp);
+	if( s != BF_STATUS_SUCCESS ) return s;
+	coherent_dedisp_chirp_kernel<<<cd_grid(nws), 256, 0, st>>>(P, nrows, nfine);
+	count_launch();
+	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
+	if( nfine == 1 ) {
+		s = bfFftExecute(plan->fft, &seg, &seg, 1, tmp, plan->fft_tmp);
+	} else {
+		const BFarray blocks = cd_seg_array(P.ws, nrows * nseg * nfine, nf);
+		s = bfFftExecute(plan->fine, &blocks, &blocks, 1, tmp, plan->fine_tmp);
+	}
+	if( s != BF_STATUS_SUCCESS ) return s;
+	const long nthread = nrows / npol * nfine * (ntime / q);
+	if( npol == 1 ) coherent_filterbank_detect_kernel<1><<<cd_grid(nthread), 256, 0, st>>>(F, nrows);
+	else            coherent_filterbank_detect_kernel<2><<<cd_grid(nthread), 256, 0, st>>>(F, nrows);
 	count_launch();
 	BFB_CUDA(cudaGetLastError(), BF_STATUS_INTERNAL_ERROR);
 	return BF_STATUS_SUCCESS;
@@ -465,6 +870,12 @@ BFstatus bfCoherentDedispGetOverlap(BFcoherentdedisp plan, BFsize* noverlap) {
 BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarray const* out,
                                  void* exec_storage, BFsize* exec_storage_size) {
 	BFB_TRY(return cd_execute(plan, in, out, exec_storage, exec_storage_size));
+}
+
+BFstatus bfCoherentDedispFilterbank(BFcoherentdedisp plan, BFarray const* in, int nfine, int mode,
+                                    int nint, BFarray const* out,
+                                    void* exec_storage, BFsize* exec_storage_size) {
+	BFB_TRY(return cfb_execute(plan, in, nfine, mode, nint, out, exec_storage, exec_storage_size));
 }
 
 BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan) { return destroy_handle(plan); }

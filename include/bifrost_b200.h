@@ -493,6 +493,49 @@ BFstatus bfCoherentDedispExecute(BFcoherentdedisp plan, BFarray const* in, BFarr
                                  void* exec_storage, BFsize* exec_storage_size);
 BFstatus bfCoherentDedispDestroy(BFcoherentdedisp plan);
 
+/* Coherent filterbank: dedisperse, channelise, detect and integrate in one
+ * pass, with an initialised BFcoherentdedisp plan (nchan, f0, df, DM, N and
+ * the overlap M unchanged).  The cf32 voltages are never written.
+ * in [nchan, nb, ntime] ci4 / ci8 / ci16 / cf32 in device space, strides and
+ *   dtypes as bfCoherentDedispExecute.
+ * mode as bfDetect: 0 scalar (each of the nb rows detected on its own, P = nb);
+ *   2 stokes, 3 stokes_i, 4 coherence take nb = 2 (row 0 x, row 1 y) and
+ *   P = nprod (4, 1, 4).  Jones or an unknown mode: BF_STATUS_UNSUPPORTED.
+ * out f32 [nchan nfine, P, ntime / (nfine nint)], strides positive multiples
+ *   of 4 bytes, only written.  Row i = c nfine + j is fine channel j of coarse
+ *   channel c, centred on f0' + i df' with df' = df / nfine and
+ *   f0' = f0 - df/2 + df'/2; its sample interval is nfine / |df| us before
+ *   integration.
+ * Fine channels: with Nf = N / nfine, fine channel j takes the Nf bins
+ *   k = (N/2 + j Nf + q) mod N, q = 0..Nf-1, of each segment's spectrum
+ *   (contiguous in natural order) and z_j[m] = sum_q Y[k(q)] exp(+2 pi i q m / Nf),
+ *   Y = H_j FFT_N(x_seg) / N, an unnormalised inverse Nf-point transform.
+ *   H_j is the chirp above with f_top replaced by the fine channel's own top
+ *   edge f_top,j = f_c,j + |df'|/2 (a linear phase in nu), so every fine
+ *   channel is aligned to its own top edge; the delays between fine channels
+ *   remain.  nfine = 1 is bfCoherentDedispExecute's filter: |z[m]| = |y[m]|.
+ * Segments: q = nfine nint, step S = q floor((N - M) / q); segments start at
+ *   0, S, 2S, .. while s < ntime (zeros past the end) and keep fine samples
+ *   [0, S / nfine), so an output never straddles two segments.  S = L when q
+ *   divides N - M.
+ * Detection uses bfDetect's arithmetic; the nint detected samples of each
+ * output are summed left to right in fp32, as bfReduce does.  With nfine = 1
+ * and S = L the result is, bit for bit,
+ *   bfCoherentDedispExecute(plan, in, Y); bfDetect(Y, D, mode, 1);
+ *   bfReduce(D, out, BF_REDUCE_SUM)      (over time by nint; none at nint 1).
+ * BF_STATUS_INVALID_ARGUMENT unless nfine is a power of two with
+ * N / nfine >= 256, nint >= 1 and nfine nint <= N - M; BF_STATUS_INVALID_SHAPE
+ * when ntime % (nfine nint) != 0, nb != 2 in a polarised mode or out's shape
+ * is wrong; BF_STATUS_UNSUPPORTED_DTYPE when out is not f32; otherwise what
+ * bfCoherentDedispExecute returns for the same in.  N <= 4096 runs one fused
+ * kernel and needs no N-sized workspace; longer N run gather, forward bfFft,
+ * chirp, an inverse bfFft over [rows nseg nfine, Nf] and one detect kernel.
+ * Deterministic: no atomics.  exec_storage follows the FDMT's storage
+ * protocol (above). */
+BFstatus bfCoherentDedispFilterbank(BFcoherentdedisp plan, BFarray const* in, int nfine, int mode,
+                                    int nint, BFarray const* out,
+                                    void* exec_storage, BFsize* exec_storage_size);
+
 /* Pulsar folding (extension; no reference counterpart): phase-binned profiles
  * of a topocentric spin model.
  * in    [nchan, ..., ntime] u8 / u16 / f32 in device space, time unit stride,

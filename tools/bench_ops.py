@@ -2,7 +2,7 @@
 the reference's own CUDA kernels (oracle/_ref/libbifrost_ref.so, same device
 buffers, same harness) where that library provides the op.
 
-    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,fold,period_search,candidates,...]
+    python tools/bench_ops.py [--nframe 32] [--ops fdmt,transpose,fft,visibilities,beamform,correlate_storage,correlate_ci4,beamform_detect,pulse_search,sk_flag,coherent_dedisp,coherent_filterbank,fold,period_search,candidates,...]
 
 Prints one JSON line per op: ms (median of runs, CUDA events on the launching
 stream), algorithmic GB/s = in+out bytes at the C ABI / time (SURVEY 8d), and
@@ -275,6 +275,9 @@ def main():
 
     if 'coherent_dedisp' in ops:
         bench_coherent_dedisp(stream)
+
+    if 'coherent_filterbank' in ops:
+        bench_coherent_filterbank(stream)
 
     if 'fold' in ops:
         bench_fold(stream)
@@ -789,6 +792,85 @@ def bench_coherent_dedisp(stream, nrep=10):
                err_composed_vs_torch=maxrel(y_cmp, y_tor), identical=identical)
         del d_x, d_y, d_src, d_seg, d_h, seg, raw, h_t, src, dst, t_out, fft, plan
         torch.cuda.empty_cache()
+
+
+def bench_coherent_filterbank(stream, nrep=10):
+    """bfCoherentDedispFilterbank on ci8 [64 chan, 2 pol, ntime] with ntime =
+    2^20 + M rounded up to a multiple of nfine (the bench_coherent_dedisp
+    band), at DM 100 / N 4096 (fused kernel) and DM 1000 / N 65536 (bfFft
+    path), nfine 1 and 16, stokes_i and stokes, nint 1.  Timed alternately in
+    one loop with: the three calls it replaces (bfCoherentDedispExecute into
+    cf32, bfDetect; no bfReduce at nint 1), bfCoherentDedispExecute alone, and
+    a device-to-device copy of the output bytes.  Compulsory bytes: the ci8
+    input read N / S times (S the segment step) plus the f32 output; their HBM
+    share is those bytes at 3.35 TB/s (H100 SXM data sheet, 700 W) over the
+    time.  At nfine 1 the fused and three-call outputs are compared bit for
+    bit; two fused runs always are."""
+    from oracle import coherent_dedisp as ocd
+    print(json.dumps({'op': 'coherent_filterbank.device', 'gpu': gpu_name()}), flush=True)
+    nchan, npol, f0, df, nint = 64, 2, 1300.78125, 1.5625, 1
+    for dm, n in CD_CASES:
+        m = ocd.overlap(nchan, f0, df, dm)
+        for nfine in (1, 16):
+            q = nfine * nint
+            ntime = -(-((1 << 20) + m) // q) * q
+            step = q * ((n - m) // q)
+            g = torch.Generator(device='cuda').manual_seed(1)
+            raw = torch.randint(-127, 128, (nchan, npol, ntime, 2), dtype=torch.int8, device='cuda', generator=g)
+            d_x = bf.empty((nchan, npol, ntime), 'ci8', 'cuda')
+            _check(_bf.bfMemcpy(d_x.ctypes.data, _bf.BF_SPACE_CUDA, raw.data_ptr(), _bf.BF_SPACE_CUDA, raw.numel()))
+            del raw
+            plan = bf.coherent_dedisp.CoherentDedisp()
+            plan.init(nchan, f0, df, dm, n)
+            d_y = bf.empty((nchan, npol, ntime), 'cf32', 'cuda')
+            for mode in ('stokes_i', 'stokes'):
+                shape = bf.coherent_dedisp.filterbank_shape(nchan, npol, ntime, nfine, mode, nint)
+                d_o = bf.empty(shape, 'f32', 'cuda')
+                d_d = bf.empty((nchan, shape[1], ntime), 'f32', 'cuda')
+                nbytes_out = int(np.prod(shape)) * 4
+                src = torch.empty(nbytes_out, dtype=torch.uint8, device='cuda')
+                dst = torch.empty_like(src)
+                fns = {'fused': lambda: plan.filterbank(d_x, d_o, nfine, mode, nint),
+                       'chain': lambda: (plan.execute(d_x, d_y), bf.detect(d_y, d_d, mode, 1)),
+                       'execute': lambda: plan.execute(d_x, d_y),
+                       'copy': lambda: dst.copy_(src)}
+                for _ in range(2):
+                    for fn in fns.values():
+                        fn()
+                torch.cuda.synchronize()
+                times = {k: [] for k in fns}
+                for _ in range(nrep):
+                    for key, fn in fns.items():
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record(stream)
+                        fn()
+                        e1.record(stream)
+                        torch.cuda.synchronize()
+                        times[key].append(e0.elapsed_time(e1))
+                a = np.asarray(d_o.copy('system'))
+                plan.filterbank(d_x, d_o, nfine, mode, nint)
+                bf.device.stream_synchronize()
+                fields = dict(repeatable=bool(np.array_equal(a.view(np.uint32),
+                                                             np.asarray(d_o.copy('system')).view(np.uint32))))
+                if nfine == 1:
+                    plan.execute(d_x, d_y)
+                    bf.detect(d_y, d_d, mode, 1)
+                    bf.device.stream_synchronize()
+                    fields['identical_to_chain'] = bool(np.array_equal(
+                        a.view(np.uint32), np.asarray(d_d.copy('system')).view(np.uint32)))
+                ms = {key: float(np.median(v)) for key, v in times.items()}
+                nbytes = nchan * npol * ntime * 2 * n / step + nbytes_out
+                report('coherent_filterbank ci8 %dx%dx%d DM=%g N=%d M=%d nfine=%d %s nint=%d'
+                       % (nchan, npol, ntime, dm, n, m, nfine, mode, nint), ms['fused'], nbytes,
+                       path='fused' if n <= 4096 else 'bfFft',
+                       realtime=round(ntime / (df * 1e6) / (ms['fused'] * 1e-3), 1),
+                       hbm_share=round(nbytes / 3.35e12 * 1e3 / ms['fused'], 3), compulsory_GB=round(nbytes / 1e9, 3),
+                       chain_ms=round(ms['chain'], 4), execute_ms=round(ms['execute'], 4),
+                       copy_ms=round(ms['copy'], 4), speedup_vs_chain=round(ms['chain'] / ms['fused'], 3),
+                       over_execute=round(ms['fused'] / ms['execute'], 3), **fields)
+                del d_o, d_d, src, dst
+            del d_x, d_y, plan
+            torch.cuda.empty_cache()
 
 
 FOLD_FP64_OPS = 11          # fp64 operations per sample in the phase and bin (DESIGN section 8)
